@@ -9,9 +9,9 @@ input-projection table lookup (layer 0) / hoisted input-projection GEMMs (layers
 recurrent K loop (last layer) -> 4 x 512 recurrent LSTM steps -> masked [mean|max|last] pool -> (256, 2400) f32.
 
 `batches_per_launch` (5) consecutive steps ride one ie_encoder_encode call (1280 rows): the persistent recurrent kernel
-(csrc/lstm_layer.cu) deals the (timestep, batch, column-tile) work items of the five independent batches round-robin over
-all 74 CTA pairs, so an item's inputs were finished two rounds earlier and the tensor pipe never waits for a step
-barrier.  Each step is still one batch of 256 issues with its own result rows; `single_batch` in the JSON line is the
+(csrc/lstm_layer.cu) deals the (timestep, batch, row-half, column-tile) work items of the five independent batches
+round-robin over all SMs (one CTA each), so while the items of one batch-step wait for the previous step the other
+batches' items keep the tensor cores busy.  Each step is still one batch of 256 issues with its own result rows; `single_batch` in the JSON line is the
 same measurement with one batch per launch.
 
 * `value`      : whole-job issues/s with the token ids already resident in HBM (CUDA events on the launching stream,
@@ -19,9 +19,7 @@ same measurement with one batch per launch.
                  -- weak scaling, no data-path collective -- and the timed region ends with the ONE all-gather of the
                  2400-d outputs).  The W warm-up steps are repeated until the device has been under this load for
                  `config.preroll_s` seconds (BENCH_PREROLL_S, default 2): the board runs at its power cap, the governor
-                 needs about a second after an idle -> load edge to settle, and the roofline denominator
-                 (MEASURED_PEAKS.json bf16_tflops_sustained) is itself a 4-second back-to-back figure.  The timed region
-                 is exactly K steps.
+                 needs about a second after an idle -> load edge to settle.  The timed region is exactly K steps.
 * `e2e`        : the same metric through the public bulk API on HOST token-id lists -- what df_to_embedding does after
                  tokenisation (py/code_intelligence/inference.py:171-229): bulk.encode_bulk_distributed(docs, ...) = global
                  length sort -> issue j to rank j mod G -> IssueEncoder.encode_id_list pipeline (pinned staging, H2D under
@@ -31,13 +29,17 @@ same measurement with one batch per launch.
 * `roofline`   : dominant kernel = lstm_layer_kernel on the 2400-wide layers.  achieved = algorithmic FLOPs per launch
                  (2*256*2400*9600 per batch-step x 512 steps x batches in the launch) / launch duration from CUDA events
                  recorded inside ie_encoder_encode around it (ie_encoder_last_phase_ms; average of the three 2400-wide
-                 layers of the last timed call).  peak = MEASURED_PEAKS.json bf16_tflops_sustained.
+                 layers of the last timed call).  peak = MEASURED_PEAKS.json bf16_tflops_sustained when that file
+                 exists, else the H100 SXM data sheet's dense bf16 rate (989 TFLOP/s at 700 W).
 * `cpu_baseline`: the CPU oracle (oracle/awd_lstm_ref.py, torch nn.LSTM fp32 == the modules the reference's fastai
                  model wraps) timed on this box's host cores on a bounded sample (>= 32 issues).
 * `--impl reference`: times that CPU path alone (the reference's own encoder is not installable: fastai/spaCy absent,
                  no network -- see DESIGN.md); each step is a bounded sample (>= 32 issues) of the same workload.
 * `extra`      : fp32-accurate mode (IE_CFG_FP32), the north star's literal 3-layer shape (N3), the device-resident MLP
                  head (configs[4]) and a var-len bulk run checked bit for bit against a single-GPU encode.
+* `--dump-outputs DIR`: after the timed steps, rank 0 writes what the last timed step returned -- the (256, 2400) f32
+                 pooled embeddings of its batch -- to DIR/embeddings.npy.  Weights and token ids are seeded, so two
+                 builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -71,7 +73,7 @@ def measured_peaks():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -228,6 +230,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output arrays to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -258,7 +262,7 @@ def main():
     ids_all[ids_all == 1] = 0
     ids_all[:, :, 0] = 2
     ids_dev = ids_all.to(dev)
-    out_dev = torch.empty((K * B, 3 * EMB), dtype=torch.float32, device=dev)
+    out_dev = torch.empty((K * B, 3 * EMB), dtype=torch.float32, device=dev)      # the K timed steps
     gathered = torch.empty((world * K * B, 3 * EMB), dtype=torch.float32, device=dev) if world > 1 else None
     stream = torch.cuda.current_stream(dev)
 
@@ -269,6 +273,7 @@ def main():
 
     # ---- launch plan: steps are submitted kPerLaunch at a time (5 x 256 rows per ie_encoder_encode call) ----------
     kPerLaunch = max(1, enc.max_batch // B)
+    warm_dev = torch.empty((kPerLaunch * B, 3 * EMB), dtype=torch.float32, device=dev)   # warm-up / pre-roll output
     def plan(first, count, per_launch):
         # a remainder launch (count % per_launch steps) goes first, so that the LAST launch of a region -- whose
         # phase events feed the roofline -- is a full one
@@ -287,8 +292,9 @@ def main():
 
     def run_device(first, count, per_launch):
         for (i, n) in plan(first, count, per_launch):
-            enc.encode_ids_device(ids_flat_dev[i * B:(i + n) * B], len_dev2[:n * B],
-                                  out_dev[(i - W) * B:(i - W + n) * B] if i >= W else out_dev[:n * B], stream)
+            dst = out_dev[(i - W) * B:(i - W + n) * B] if i >= W else warm_dev[:n * B]
+            assert dst.shape[0] == n * B
+            enc.encode_ids_device(ids_flat_dev[i * B:(i + n) * B], len_dev2[:n * B], dst, stream)
 
     preroll_s = float(os.environ.get("BENCH_PREROLL_S", "2.0"))
 
@@ -324,6 +330,9 @@ def main():
     ms_max, launches, phases, phase_mhz = device_arm(kPerLaunch)   # five batches per launch: the bulk-encode mode
     value = world * B * K / (ms_max * 1e-3)
     single_value = world * B * K / (ms_single * 1e-3)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "embeddings.npy"), out_dev[(K - 1) * B:K * B].cpu().numpy())
 
     # ---- end-to-end arm: HOST token-id lists through the public bulk API -----------------------------------
     # every rank holds the same global list (the reference's per-repo list of numericalised issues), as the API expects
@@ -404,19 +413,14 @@ def main():
 
     if rank == 0:
         peaks = measured_peaks()
-        peak = (peaks or {}).get("bf16_tflops_sustained", 1400.0)
-        peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "fallback 1.4 PFLOP/s sustained"
+        peak = (peaks or {}).get("bf16_tflops_sustained", 989.0)
+        peak_src = ("measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks
+                    else "H100 SXM data sheet, dense bf16 at 700 W (not a measured rate)")
         batches = kPerLaunch if K >= kPerLaunch else K   # batches riding the LAST timed launch (see plan())
         step_ms = phases["steps"][:N_LAYERS - 1]
         avg_launch_ms = sum(step_ms) / len(step_ms)
         flop_per_launch = STEP_FLOP_2400 * T * batches
         achieved = flop_per_launch / (avg_launch_ms * 1e-3) / 1e12
-        traffic, traffic_src = None, None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "lstm_layer_traffic.json")))
-            traffic, traffic_src = tj["dram_bytes_per_launch"], tj.get("source")
-        except Exception:
-            pass
         line = {
             "metric": "issues/sec to 2400-d @ seq_len 512 batch 256", "value": value, "unit": "issues/s",
             "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": ms_max / K, "higher_is_better": True,
@@ -442,7 +446,7 @@ def main():
             "roofline": {"bound": "tensor", "kernel": "lstm_layer_kernel (persistent recurrent kernel, 2400-wide layers, "
                                    "%d batches in the last timed launch)" % batches,
                          "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "avg_launch_us": avg_launch_ms * 1e3, "flop_per_launch": flop_per_launch,
                          "whole_step_tflops": FLOP_PER_TOKEN * B * T / (ms_max / K * 1e-3) / 1e12,
                          "whole_step_frac": FLOP_PER_TOKEN * B * T / (ms_max / K * 1e-3) / 1e12 / peak,
@@ -542,8 +546,8 @@ def extras_rank0(enc, emb, layers, dev, R):
         flop = 2.0 * n * (d_in * 600 + 600 * 600 + 600 * 256)
         byt = n * (d_in * 4 + 256 * 4)
         peaks = measured_peaks() or {}
-        hbm = peaks.get("hbm_gbs", 6500.0)
-        tf = peaks.get("bf16_tflops_sustained", 1400.0)
+        hbm = peaks.get("hbm_gbs", 3350.0)          # H100 SXM data sheet when no measured peaks exist
+        tf = peaks.get("bf16_tflops_sustained", 989.0)
         t_hbm, t_tensor = byt / hbm / 1e6, flop / tf / 1e9          # ms at the measured peaks
         # the binding roofline is the slower of the two: at D_in >= 1600 the three bf16 GEMMs (tensor) outlast the
         # f32 X read + probability write (HBM)
@@ -553,7 +557,7 @@ def extras_rank0(enc, emb, layers, dev, R):
             roof = {"bound": "hbm", "achieved": byt / ms / 1e6, "peak": hbm, "unit": "GB/s", "frac": t_hbm / ms}
         roof["hbm_frac"] = t_hbm / ms
         roof["note"] = ("algorithmic FLOPs 2 n (D_in 600 + 600 600 + 600 256); algorithmic bytes = f32 X in + f32 "
-                        "probabilities out; peaks from MEASURED_PEAKS.json")
+                        "probabilities out; peaks from MEASURED_PEAKS.json, else the H100 SXM data sheet")
         out[f"mlp_{d_in}"] = {"rows_per_s": n / ms * 1e3, "labels_per_s": n * 256 / ms * 1e3, "ms": ms,
                               "tflops": flop / ms / 1e9, "hbm_gbs": byt / ms / 1e6, "roofline": roof}
         head.close()

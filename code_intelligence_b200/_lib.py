@@ -1,7 +1,7 @@
 """ctypes binding of libissue_emb_b200.so (C ABI: include/issue_emb_b200.h).
 
 There is deliberately NO fallback: if the CUDA library is missing or cannot be loaded this module raises, and
-every entry point fails when no sm_100 device is present.
+every entry point fails when no sm_90 (H100) device is present.
 """
 from __future__ import annotations
 
@@ -56,7 +56,7 @@ _lib = None
 
 
 def build(verbose: bool = False) -> Path:
-    """Compile the CUDA sources for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA sources for sm_90a (nvcc cross-compiles without a GPU)."""
     r = subprocess.run(["make", "-C", str(_PKG / "csrc"), "-j8"], capture_output=True, text=True)
     if verbose or r.returncode != 0:
         print(r.stdout[-4000:])

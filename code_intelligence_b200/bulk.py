@@ -43,7 +43,7 @@ def encode_sorted_batches(docs: List[np.ndarray], encode_padded: Callable, pad_i
     ``RuntimeError`` (CUDA OOM, :214-223) halve ``bs`` and retry the same position -- re-raised as ``Exception`` at
     bs == 1 -- and finally unsort with argsort(argsort) (:226).
 
-    ``coalesce=True``: consecutive sorted batches are merged into device calls of ``max_bs`` rows.  On the B200 path a
+    ``coalesce=True``: consecutive sorted batches are merged into device calls of ``max_bs`` rows.  On the GPU path a
     row's result does not depend on its batch mates or on the padded length (bit-exact, tests/test_gpu_parity.py), so
     ``bs`` -- a memory knob of the reference, default 100 -- only decides how many rows ride one launch; merging keeps
     the results and lets a caller with the reference's default arguments reach full 1280-row launches."""

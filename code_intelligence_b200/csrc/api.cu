@@ -79,7 +79,7 @@ struct DevBuf {
 
 struct Layer {
   int in = 0, out = 0;      // logical dims
-  int u = 32, n_cta = 0;    // hidden units per weight slice (CTA), slices (even: CTA pairs own two)
+  int u = 32, n_cta = 0;    // hidden units per weight slice, slices (even: a 256-column tile owns two)
   int out_pad = 0;          // n_cta * u
   int kin_pad = 0;          // padded K of the input projection
   int kh_pad = 0;           // padded K of the recurrent projection
@@ -93,20 +93,20 @@ struct Layer {
 
 struct ie_encoder {
   ie_config cfg{};
-  int num_sms = 148;
+  int num_sms = 132;
   int e_pad = 0;  // emb_sz rounded up to 64
-  // one weight layout: slices of u = 32 hidden units, rows [slice][unit][gate]; a CTA pair owns two slices = one
-  // N = 256 accumulator tile (lstm_layer.cu), the fallback kernel one slice per CTA (lstm.cu)
+  // one weight layout: slices of u = 32 hidden units (slice_perm); two slices = one N = 256 accumulator tile of the
+  // recurrent kernel (lstm_layer.cu)
   std::vector<Layer> layers;
   int segs = 1;            // 1: bf16 operands; 3: split-bf16 ("fp32-accurate", IE_CFG_FP32)
   int gate_mode = 2;       // lstm_common.cuh: 2 tanh.approx, 1 ex2+rcp, 0 IEEE
   int gx_bf16 = 1;         // input projections (Gx, per-token table) stored as 16-bit floats -- IEEE half -- instead of f32
                            // (f32 in the fp32-accurate mode)
-  int use_persistent = 1;  // cooperative persistent kernel; 0 (IE_SEQ=0 or not co-resident): per-timestep fallback
+  int use_persistent = 1;  // cooperative persistent launch; 0 (IE_SEQ=0 or not co-resident): one launch per timestep
   int persist_checked = 0;
   int cooperative = 1;     // launch attribute (IE_COOP=0: plain launch, co-residency by the occupancy check only)
-  int use_mc = 0;          // IE_MC=1: sibling CTA pairs share h tiles by TMA multicast (clusters of four)
-  int mc_pairs = 0;        // pairs co-resident in clusters of four
+  int use_mc = 0;          // IE_MC=1: sibling CTAs share h tiles by TMA multicast (clusters of two)
+  int mc_ctas = 0;         // CTAs co-resident in clusters of two
   int batches = 5;         // batches of 256 rows one launch takes (IE_BATCHES, <= kMaxBatches)
   int fuse_last = 1;       // the last layer's input projection rides its recurrent K loop (lstm_layer.cu FUSE) instead of a
                            // hoisted GEMM + Gx round trip (IE_FUSE_LAST=0: hoisted like the other layers)
@@ -146,7 +146,7 @@ struct ie_encoder {
 
 struct ie_mlp {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   std::vector<int> dims;
   struct L {
     int k_pad = 0, n_pad = 0, bn = 0;
@@ -178,7 +178,7 @@ int plan_layers(ie_encoder* h) {
     L.out = (l == c.n_layers - 1) ? c.emb_sz : c.n_hid;
     L.u = 32;
     L.n_cta = (L.out + L.u - 1) / L.u;
-    if (L.n_cta & 1) ++L.n_cta;  // CTA pairs: the last pair's second slice is pure padding
+    if (L.n_cta & 1) ++L.n_cta;  // whole tiles: the last tile's second slice is pure padding
     L.out_pad = L.n_cta * L.u;
     L.kin_pad = prev_pad;
     L.kh_pad = L.out_pad;        // multiple of 64
@@ -188,15 +188,17 @@ int plan_layers(ie_encoder* h) {
   return IE_OK;
 }
 
-// torch gate-major rows [4*out] -> sliced rows [slice][unit][gate]; -1 marks zero padding rows
+// torch gate-major rows [4*out] -> the recurrent kernel's column order; -1 marks zero padding rows.  Units go in groups
+// of four = 16 columns; unit q of a group has (i, f) at columns 2q, 2q+1 and (g, o) at 8+2q, 9+2q -- exactly the
+// columns one thread holds in a wgmma accumulator fragment (lstm_layer.cu), so a thread owns all four gates of a unit.
 std::vector<int> slice_perm(const Layer& L) {
   std::vector<int> perm(4 * static_cast<size_t>(L.out_pad));
-  for (int j = 0; j < L.n_cta; ++j)
-    for (int i = 0; i < L.u; ++i)
-      for (int g = 0; g < 4; ++g) {
-        const int unit = j * L.u + i;
-        perm[(static_cast<size_t>(j) * L.u + i) * 4 + g] = unit < L.out ? g * L.out + unit : -1;
-      }
+  for (int unit = 0; unit < L.out_pad; ++unit)
+    for (int g = 0; g < 4; ++g) {
+      const int q = unit & 3;
+      const size_t col = static_cast<size_t>(unit >> 2) * 16 + (g < 2 ? 2 * q + g : 8 + 2 * q + (g - 2));
+      perm[col] = unit < L.out ? g * L.out + unit : -1;
+    }
   return perm;
 }
 
@@ -333,8 +335,8 @@ int check_persistent(ie_encoder* h, cudaStream_t s) {
     const Layer& L = h->layers[0];
     q.T = 1; q.ng = 1; q.u = L.u; q.n_cta = L.n_cta; q.out_pad = L.out_pad; q.kh_pad = L.kh_pad; q.segs = 1;
     q.num_sms = h->num_sms; q.check_only = 1; q.mc = 1; q.gx_bf16 = 1;
-    if (ie::launch_lstm_layer(q, s) == cudaSuccess) h->mc_pairs = ie::lstm_layer_max_pairs() & ~1;
-    if (h->mc_pairs < 2) h->use_mc = 0;
+    if (ie::launch_lstm_layer(q, s) == cudaSuccess) h->mc_ctas = ie::lstm_layer_max_ctas() & ~1;
+    if (h->mc_ctas < 2) h->use_mc = 0;
   }
   cudaGetLastError();
   h->persist_checked = 1;
@@ -363,8 +365,9 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
     return fail(IE_ERR_OOM, "B_pad*T = %lld tokens exceeds the workspace cap %lld; use a smaller batch",
                 static_cast<long long>(b_pad) * T, cap);
   CK(cudaSetDevice(c.device));
-  // <= 2^21 (timestep, row) pairs of Gx at once (40 GB as fp16 at H = 2400); half of that with f32 projections
-  long long chunk_T = std::max<long long>(1, ((h->gx_bf16 ? 2ll : 1ll) << 20) / b_pad);
+  // <= 2^20 (timestep, row) pairs of Gx at once (20 GB as fp16 at H = 2400, plus 10 GB of hidden-state rings: well
+  // inside the H100's 80 GB); half of that with f32 projections
+  long long chunk_T = std::max<long long>(1, ((h->gx_bf16 ? 2ll : 1ll) << 19) / b_pad);
   if (h->chunk_t > 0) chunk_T = h->chunk_t;
   chunk_T = std::min<long long>(chunk_T, T);
   const bool proj = proj_usable(h);
@@ -440,10 +443,10 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
                                h->y_ld, 64, 128));
       if (fused)
         CK(ie::make_tmap_bf16_2d(&tm_w, L.w_cat.p, static_cast<uint64_t>(L.kin_pad + L.kh_pad), 4ull * L.out_pad,
-                                 static_cast<uint64_t>(L.kin_pad + L.kh_pad), 64, 128));
+                                 static_cast<uint64_t>(L.kin_pad + L.kh_pad), 64, 256));
       else
         CK(ie::make_tmap_bf16_2d(&tm_w, L.w_hh.p, static_cast<uint64_t>(ring_mul) * L.kh_pad, 4ull * L.out_pad,
-                                 static_cast<uint64_t>(ring_mul) * L.kh_pad, 64, 128));
+                                 static_cast<uint64_t>(ring_mul) * L.kh_pad, 64, 256));
       CUtensorMap tm_h64 = tm_h;
       CUtensorMap tm_x = tm_h;
       if (fused)
@@ -469,35 +472,35 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
       }
       if ((rc = mark(h, 2 + 2 * l, s)) != IE_OK) return rc;
 
+      if (persistent) CK(cudaMemsetAsync(h->step_done.p, 0, static_cast<size_t>(Tc) * ng * sizeof(unsigned), s));
+      ie::LstmLayerArgs q{};
+      q.tm_h = tm_h; q.tm_w = tm_w; q.tm_h64 = tm_h64; q.mc = h->use_mc; q.mc_ctas = h->mc_ctas;
+      q.tm_x = tm_x; q.pre_nkb = fused ? L.kin_pad / 64 : 0; q.bias = L.bias.as<float>();
+      q.gx = from_table ? h->proj.p : h->gx.p;
+      q.tok = from_table ? h->tok.as<int>() : nullptr;
+      q.c = cstate; q.y = ybuf;
+      q.raw = (last && raw_out != nullptr) ? h->raw.as<float>() : nullptr;
+      q.pool_sum = (last && pooled) ? h->pool_sum.as<float>() : nullptr;
+      q.pool_max = h->pool_max.as<float>(); q.pool_last = h->pool_last.as<float>();
+      q.lengths = h->lengths.as<int>();
+      q.step_done = h->step_done.as<unsigned>();
+      q.abort_flag = h->err.as<unsigned>() + 1; q.spin_limit = h->spin_limit;
+      q.T = Tc; q.t0 = static_cast<int>(t0); q.T_total = T; q.ng = ng;
+      q.u = L.u; q.n_cta = L.n_cta; q.out_pad = L.out_pad; q.kh_pad = L.kh_pad;
+      q.ldy = h->y_ld; q.raw_ld = L.out_pad;
+      q.gate_mode = h->gate_mode; q.gx_bf16 = h->gx_bf16; q.segs = h->segs;
+      q.num_sms = h->num_sms; q.check_only = 0; q.cooperative = h->cooperative; q.fault = h->fault;
+      q.diag = h->diag.as<long long>() + 8 * l;
+      q.trace = nullptr;
       if (persistent) {
-        CK(cudaMemsetAsync(h->step_done.p, 0, static_cast<size_t>(Tc) * ng * sizeof(unsigned), s));
-        ie::LstmLayerArgs q{};
-        q.tm_h = tm_h; q.tm_w = tm_w; q.tm_h64 = tm_h64; q.mc = h->use_mc; q.mc_pairs = h->mc_pairs;
-        q.tm_x = tm_x; q.pre_nkb = fused ? L.kin_pad / 64 : 0; q.bias = L.bias.as<float>();
-        q.gx = from_table ? h->proj.p : h->gx.p;
-        q.tok = from_table ? h->tok.as<int>() : nullptr;
-        q.c = cstate; q.y = ybuf;
-        q.raw = (last && raw_out != nullptr) ? h->raw.as<float>() : nullptr;
-        q.pool_sum = (last && pooled) ? h->pool_sum.as<float>() : nullptr;
-        q.pool_max = h->pool_max.as<float>(); q.pool_last = h->pool_last.as<float>();
-        q.lengths = h->lengths.as<int>();
-        q.step_done = h->step_done.as<unsigned>();
-        q.abort_flag = h->err.as<unsigned>() + 1; q.spin_limit = h->spin_limit;
-        q.T = Tc; q.t0 = static_cast<int>(t0); q.T_total = T; q.ng = ng;
-        q.u = L.u; q.n_cta = L.n_cta; q.out_pad = L.out_pad; q.kh_pad = L.kh_pad;
-        q.ldy = h->y_ld; q.raw_ld = L.out_pad;
-        q.gate_mode = h->gate_mode; q.gx_bf16 = h->gx_bf16; q.segs = h->segs;
-        q.num_sms = h->num_sms; q.check_only = 0; q.cooperative = h->cooperative; q.fault = h->fault;
-        q.diag = h->diag.as<long long>() + 8 * l;
-        q.trace = nullptr;
         if (l == h->trace_layer && t0 == 0) {
-          const int pairs = ie::lstm_layer_pairs(q);
-          const long long items = (static_cast<long long>(Tc) * ng * (L.n_cta / 2) + pairs - 1) / pairs;
-          CK(h->trace.reserve(static_cast<size_t>(2 * pairs) * items * 12 * sizeof(long long), true));
+          const int ctas = ie::lstm_layer_ctas(q);
+          const long long items = (static_cast<long long>(Tc) * ng * L.n_cta + ctas - 1) / ctas;
+          CK(h->trace.reserve(static_cast<size_t>(ctas) * items * 12 * sizeof(long long), true));
           q.trace = h->trace.as<long long>();
           q.trace_items = static_cast<int>(items);
           h->trace_T = static_cast<int>(items);
-          h->trace_ctas = 2 * pairs;
+          h->trace_ctas = ctas;
         }
         cudaError_t e = ie::launch_lstm_layer(q, s);
         if (e == cudaErrorCooperativeLaunchTooLarge) {
@@ -508,26 +511,13 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
         CK(e);
         h->launches += 1;
       } else {
-        ie::LstmStepArgs a{};
-        a.tm_h = tm_h; a.tm_w = tm_w;
-        a.gx = from_table ? h->proj.p : h->gx.p;
-        a.tok = from_table ? h->tok.as<int>() : nullptr;
-        a.c = cstate; a.y = ybuf;
-        a.raw = (last && raw_out != nullptr) ? h->raw.as<float>() : nullptr;
-        a.pool_sum = (last && pooled) ? h->pool_sum.as<float>() : nullptr;
-        a.pool_max = h->pool_max.as<float>(); a.pool_last = h->pool_last.as<float>();
-        a.lengths = h->lengths.as<int>();
-        a.abort_flag = h->err.as<unsigned>() + 1; a.spin_limit = h->spin_limit;
-        a.t0 = static_cast<int>(t0); a.T_total = T; a.b_pad = b_pad;
-        a.u = L.u; a.n_cta = L.n_cta; a.out_pad = L.out_pad; a.kh_pad = L.kh_pad;
-        a.ldy = h->y_ld; a.raw_ld = L.out_pad;
-        a.gate_mode = h->gate_mode; a.gx_bf16 = h->gx_bf16; a.segs = h->segs;
-        for (int t = 0; t < Tc; ++t)
-          for (int g = 0; g < ng; ++g) {
-            a.t = t; a.g = g;
-            CK(ie::launch_lstm_step(a, s));
-          }
-        h->launches += static_cast<int64_t>(Tc) * ng;
+        q.single_step = 1;
+        q.diag = nullptr;
+        for (int t = 0; t < Tc; ++t) {
+          q.t_step = t;
+          CK(ie::launch_lstm_layer(q, s));
+        }
+        h->launches += Tc;
       }
       if (t0 + Tc < T)  // carry h of the chunk's last step into the next chunk
         CK(cudaMemcpyAsync(carry, ybuf + static_cast<size_t>(Tc) * b_pad * h->y_ld, slot_bytes, cudaMemcpyDeviceToDevice, s));
@@ -612,7 +602,7 @@ int ie_encoder_create(const ie_config* cfg, ie_encoder** out) {
   int major = 0, sms = 0;
   CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, cfg->device));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device));
-  if (major != 10) return fail(IE_ERR_CUDA, "device compute capability %d.x is not sm_100 (B200)", major);
+  if (major != 9) return fail(IE_ERR_CUDA, "device compute capability %d.x is not sm_90 (H100)", major);
   ie_encoder* h = new ie_encoder();
   h->cfg = *cfg;
   h->num_sms = sms;
@@ -812,7 +802,7 @@ int ie_mlp_create(int32_t n_layers, const int32_t* dims, int32_t device, ie_mlp*
   int major = 0, sms = 0;
   CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-  if (major != 10) return fail(IE_ERR_CUDA, "device compute capability %d.x is not sm_100 (B200)", major);
+  if (major != 9) return fail(IE_ERR_CUDA, "device compute capability %d.x is not sm_90 (H100)", major);
   ie_mlp* m = new ie_mlp();
   m->device = device;
   m->num_sms = sms;
@@ -822,9 +812,8 @@ int ie_mlp_create(int32_t n_layers, const int32_t* dims, int32_t device, ie_mlp*
   for (int l = 0; l < n_layers; ++l) {
     ie_mlp::L& L = m->layers[l];
     L.k_pad = static_cast<int>(round_up(dims[l], 64));
-    // N tile: a tcgen05.mma costs about the same whatever its N (profiles/README.md), so wide layers use the full N = 256
-    // (a 600-wide hidden layer is padded to 768 = 3 tiles: 123 instead of 185 instruction slots per 128-row tile for the
-    // (1600, 600, 600, 256) head) and narrow ones a single tile
+    // N padding: the GEMM's tiles are 256 wide (a 600-wide hidden layer is padded to 768 = 3 tiles), narrow layers are
+    // padded to 16 columns and the rest of their single tile reads zero weights
     const int n16 = static_cast<int>(round_up(dims[l + 1], 16));
     L.bn = n16 >= 256 ? 256 : n16;
     L.n_pad = static_cast<int>(round_up(dims[l + 1], L.bn));
@@ -878,9 +867,6 @@ int ie_mlp_predict_proba(ie_mlp* m, const float* X, int32_t n, float* probs, int
   const ie_mlp::L& LL = m->layers[nl - 1];
   // the last GEMM writes straight into the caller's array when its row pitch is a legal store width
   const bool direct_out = dev && n_labels % 16 == 0 && n_labels == LL.n_pad;
-  // (Converting chunk k+1 on a side stream under the GEMMs of chunk k was measured: 6.79 vs 6.84 ms per 2^20 rows at
-  // D_in = 2400 -- the HBM-bound convert pass and the tensor-bound GEMMs share the board's power budget, not only the SMs;
-  // profiles/README.md.)
   CK(m->act[0].reserve(static_cast<size_t>(chunk) * m->act_ld * sizeof(__nv_bfloat16), true));
   CK(m->act[1].reserve(static_cast<size_t>(chunk) * m->act_ld * sizeof(__nv_bfloat16), true));
   CK(m->xb.reserve(static_cast<size_t>(chunk) * m->act_ld * sizeof(__nv_bfloat16), true));
@@ -888,9 +874,8 @@ int ie_mlp_predict_proba(ie_mlp* m, const float* X, int32_t n, float* probs, int
   if (!dev) CK(m->xf.reserve(static_cast<size_t>(chunk) * d_in * sizeof(float)));
   for (long long r0 = 0; r0 < n; r0 += chunk) {
     const int rows = static_cast<int>(std::min<long long>(chunk, n - r0));
-    // whole M = 256 tiles when there are enough of them for the CTA-pair GEMM (rows past `rows` hold stale finite data
-    // and are never stored)
-    const int m_pad = static_cast<int>(rows >= 256 * 40 ? round_up(rows, 256) : round_up(rows, 128));
+    // whole M = 128 tiles (rows past `rows` hold stale finite data and are never stored)
+    const int m_pad = static_cast<int>(round_up(rows, 128));
     const float* xsrc = X + r0 * d_in;
     if (!dev) {
       CK(cudaMemcpyAsync(m->xf.p, xsrc, static_cast<size_t>(rows) * d_in * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -993,7 +978,7 @@ int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, 
                   float* d, int32_t device) {
   if (a == nullptr || b == nullptr || d == nullptr || M < 1 || N < 1 || K < 1) return fail(IE_ERR_INVALID, "bad argument");
   CK(cudaSetDevice(device));
-  int sms = 148;
+  int sms = 132;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
   const int m_pad = static_cast<int>(round_up(M, 128)), k_pad = static_cast<int>(round_up(K, 64));
   const int n16 = static_cast<int>(round_up(N, 16));

@@ -1,21 +1,18 @@
-// Persistent tcgen05 GEMM:  D[M, N] = act(A[M, K] * B[N, K]^T + bias[N])
+// Persistent wgmma GEMM:  D[M, N] = act(A[M, K] * B[N, K]^T + bias[N])
 //
 //   A, B : bf16, K-major (row-major with K contiguous), K padded to a multiple of 64 and physically
-//          zero-filled, rows padded to whole tiles -> no reliance on TMA out-of-bounds fill.
-//   D    : f32 or bf16, row-major with leading dimension ldd.
+//          zero-filled, A rows padded to whole 128-row tiles; B rows past n_pad read as zeros (TMA out-of-bounds fill).
+//   D    : f32, bf16 or fp16, row-major with leading dimension ldd.
 //
 // Used for (i) the hoisted LSTM input projections  Gx = X * W_ih^T + (b_ih + b_hh)  over all T*B rows at
 // once (the non-recurrent 46 % of the encoder FLOPs; reference: fastai AWD_LSTM -> torch nn.LSTM called at
 // Issue_Embeddings/flask_app/inference.py:57,68) and (ii) the Label_Microservice MLP layers
 // (py/label_microservice/mlp.py:63 -> sklearn predict_proba).
 //
-// Structure (one CTA per SM, 256 threads, warp-specialised):
-//   warp 0      TMA producer: A tile 128x64 and B tile bn x 64 per stage, 128B swizzle, mbarrier complete_tx
-//   warp 1      UMMA issuer : tcgen05.mma kind::f16 M=128 N=bn K=16, accumulators in TMEM (double buffered)
-//   warp 2      TMEM allocator
-//   warps 4..7  epilogue    : tcgen05.ld -> +bias -> activation -> global stores; overlaps the next tile's MMAs
-#include <cstdlib>
-
+// Structure (one CTA per SM, 384 threads, warp-specialised, tiles of 128 x 256):
+//   warpgroup 0      TMA producer (one thread): A tile 128x64 and B tile 256x64 per stage, 128B swizzle, mbarrier complete_tx
+//   warpgroups 1, 2  consumers: wgmma m64n256k16 into registers (64 rows each), then +bias -> activation -> global
+//                    stores; the producer fills the next tile's stages meanwhile
 #include <cuda_fp16.h>
 #include <type_traits>
 
@@ -32,29 +29,27 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
 }
 
 constexpr int kBlockM = 128;
+constexpr int kBlockN = 256;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 B = one swizzle atom
-constexpr int kGemmThreads = 256;
+constexpr int kGemmThreads = 384;
+constexpr int kGemmStages = 4;
+constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
+constexpr uint32_t kBBytes = kBlockN * kBlockK * 2;
+constexpr uint32_t kGemmStageBytes = kABytes + kBBytes;
 
 template <typename OutT, int ACT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, OutT* __restrict__ D,
                  const float* __restrict__ bias, int m_store, int n_store, long long ldd, int num_m_blocks,
-                 int num_n_blocks, int num_k_blocks, int bn, int stages, int panel, int segs, int k_pad,
-                 unsigned* abort_flag, long long spin_limit, long long* diag) {
+                 int num_n_blocks, int num_k_blocks, int panel, int segs, int k_pad, unsigned* abort_flag,
+                 long long spin_limit, long long* diag) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
 
-  const uint32_t a_bytes = kBlockM * kBlockK * 2;
-  const uint32_t b_bytes = static_cast<uint32_t>(bn) * kBlockK * 2;
-  const uint32_t stage_bytes = a_bytes + b_bytes;  // bn % 8 == 0 -> multiple of 1024
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + static_cast<size_t>(stages) * stage_bytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + stages;
-  uint64_t* tfull_bar = bars + 2 * stages;
-  uint64_t* tempty_bar = bars + 2 * stages + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * stages + 4);
-  uint32_t* abort_s = tmem_slot + 1;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kGemmStages * kGemmStageBytes);
+  uint64_t* empty_bar = full_bar + kGemmStages;
+  uint32_t* abort_s = reinterpret_cast<uint32_t*>(empty_bar + kGemmStages);
   const Abort ab{abort_s, abort_flag, spin_limit};
   const int nkt = num_k_blocks * segs;  // split-bf16: K loop over [A_hi | A_lo | A_hi] x [B_hi | B_hi | B_lo]
 
@@ -72,22 +67,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   }
   if (warp == 1 && lane == 0) {
-    for (int s = 0; s < stages; ++s) {
+    for (int s = 0; s < kGemmStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], 128);
+      mbar_init(&empty_bar[s], 2);
     }
     *abort_s = 0;
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_tiles = num_m_blocks * num_n_blocks;
   const int panel_tiles = panel * num_n_blocks;
@@ -102,8 +89,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     m_blk = m0 + (r - n_blk * mcnt);
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles && !aborted(ab); tile += gridDim.x) {
@@ -112,346 +99,79 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int kb = 0; kb < nkt; ++kb) {
           const int seg = kb / num_k_blocks, r = kb - seg * num_k_blocks;
           mbar_wait(&empty_bar[stage], phase ^ 1, ab);
-          uint8_t* sa = smem + static_cast<size_t>(stage) * stage_bytes;
-          mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
+          uint8_t* sa = smem + static_cast<size_t>(stage) * kGemmStageBytes;
+          mbar_arrive_expect_tx(&full_bar[stage], kGemmStageBytes);
           tma_load_2d(sa, &tmA, &full_bar[stage], (seg == 1 ? k_pad : 0) + r * kBlockK, m_blk * kBlockM, kEvictNormal);
-          tma_load_2d(sa + a_bytes, &tmB, &full_bar[stage], (seg == 2 ? k_pad : 0) + r * kBlockK, n_blk * bn, kEvictLast);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
+          tma_load_2d(sa + kABytes, &tmB, &full_bar[stage], (seg == 2 ? k_pad : 0) + r * kBlockK, n_blk * kBlockN,
+                      kEvictLast);
+          if (++stage == kGemmStages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(kBlockM, bn);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles && !aborted(ab); tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1, ab);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(acc * bn);
-        for (int kb = 0; kb < nkt; ++kb) {
-          mbar_wait(&full_bar[stage], phase, ab);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + static_cast<size_t>(stage) * stage_bytes);
-          const uint64_t da = umma_desc_sw128(sa);
-          const uint64_t db = umma_desc_sw128(sa + a_bytes);
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) {
-            // advance 16 bf16 = 32 B inside the swizzle atom: +2 in the (addr >> 4) field
-            umma_bf16(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp - 4;  // TMEM lane quarter == warp % 4
-    int acc = 0;
-    uint32_t acc_phase = 0;
+  } else {
+    const int wg = (warp - 4) >> 2;
+    const int q = lane & 3;
+    const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const uint32_t smem_base = smem_u32(smem);
+    const bool signal = (threadIdx.x & 127) == 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    float d[128];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int m_blk, n_blk;
       decode(tile, m_blk, n_blk);
-      mbar_wait(&tfull_bar[acc], acc_phase, ab);
-      tc_fence_after();
-      const int row = m_blk * kBlockM + q * 32 + lane;
-      const bool row_ok = row < m_store;
-      OutT* drow = D + static_cast<long long>(row) * ldd;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * bn);
-      for (int c = 0; c < bn; c += 16) {
-        uint32_t r[16];
-        tmem_ld16(taddr + c, r);
-        tmem_ld_wait();
-        const int n = n_blk * bn + c;
-        if (row_ok && n < n_store) {
-          float v[16];
+      int prev = -1;
+      for (int kb = 0; kb < nkt; ++kb) {
+        mbar_wait(&full_bar[stage], phase, ab);
+        const uint32_t sa = smem_base + stage * kGemmStageBytes;
+        const uint64_t da = wgmma_desc_sw128(sa + wg * (kABytes / 2));
+        const uint64_t db = wgmma_desc_sw128(sa + kABytes);
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float x = __uint_as_float(r[j]);
-            if (bias != nullptr) x += __ldg(bias + n + j);
-            if (ACT == 1) x = fmaxf(x, 0.0f);
-            if (ACT == 2) x = sigmoid_acc(x);
-            v[j] = x;
-          }
-          if constexpr (sizeof(OutT) == 4) {
-#pragma unroll
-            for (int j = 0; j < 2; ++j)
-              st_global_v8(drow + n + 8 * j, __float_as_uint(v[8 * j]), __float_as_uint(v[8 * j + 1]),
-                           __float_as_uint(v[8 * j + 2]), __float_as_uint(v[8 * j + 3]), __float_as_uint(v[8 * j + 4]),
-                           __float_as_uint(v[8 * j + 5]), __float_as_uint(v[8 * j + 6]), __float_as_uint(v[8 * j + 7]));
-          } else if constexpr (std::is_same<OutT, __half>::value) {
-            st_global_v8(drow + n, pack_f16x2(v[0], v[1]), pack_f16x2(v[2], v[3]), pack_f16x2(v[4], v[5]),
-                         pack_f16x2(v[6], v[7]), pack_f16x2(v[8], v[9]), pack_f16x2(v[10], v[11]),
-                         pack_f16x2(v[12], v[13]), pack_f16x2(v[14], v[15]));
-          } else {
-            st_global_v8(drow + n, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
-                         pack_bf16x2(v[6], v[7]), pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]),
-                         pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
-          }
+        for (int k = 0; k < kBlockK / 16; ++k) wgmma_m64n256k16(d, da + 2 * k, db + 2 * k, (kb | k) != 0);
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          if (signal) mbar_arrive(&empty_bar[prev]);
         }
+        prev = stage;
+        if (++stage == kGemmStages) { stage = 0; phase ^= 1; }
       }
-      tc_fence_before();
-      mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-  if (diag != nullptr && threadIdx.x == 0 && blockIdx.x == 0) {
-    unsigned long long g;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
-    diag[2] = clock64();
-    diag[3] = static_cast<long long>(g);
-  }
-}
-
-// ----------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): a cluster of two CTAs on one TPC computes a 256 x bn tile.  CTA r loads
-// rows [128r, +128) of the A tile and rows [r*bn/2, +bn/2) of the B tile; one M=256 UMMA per K=16 slice feeds both
-// tensor cores, so each SM reads A (4 KB) + half of B per instruction instead of A + all of B -- the single-CTA
-// kernel above is bound by that shared-memory operand traffic (~68 % tensor-pipe activity, profiles/README.md).
-// ----------------------------------------------------------------------------------------------
-template <typename OutT, int ACT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
-gemm_bf16_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const __grid_constant__ CUtensorMap tmD, OutT* __restrict__ D, const float* __restrict__ bias, int m_store, int n_store, long long ldd,
-                      int num_m_blocks /* of 256 rows */, int num_n_blocks, int num_k_blocks, int bn, int stages,
-                      int panel, int segs, int k_pad, unsigned* abort_flag, long long spin_limit, long long* diag,
-                      int use_tma_store) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
-
-  const uint32_t a_bytes = kBlockM * kBlockK * 2;
-  const uint32_t b_bytes = static_cast<uint32_t>(bn / 2) * kBlockK * 2;   // this CTA's half of the B tile
-  const uint32_t stage_bytes = a_bytes + b_bytes;
-  // 16-bit outputs leave through shared memory + TMA stores: 2 x (128 rows x 64 columns, 128B swizzle) staging tiles
-  const bool kTmaStore = sizeof(OutT) == 2 && use_tma_store != 0;
-  constexpr uint32_t kOutTileBytes = 128 * 128;
-  uint8_t* out_stage = smem + static_cast<size_t>(stages) * stage_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(out_stage + (kTmaStore ? 2 * kOutTileBytes : 0));
-  uint64_t* full_bar = bars;                   // leader's copy is live: 2 arrivals + both CTAs' bytes
-  uint64_t* empty_bar = bars + stages;         // per CTA, arrival = the leader's multicast commit
-  uint64_t* tfull_bar = bars + 2 * stages;     // per CTA
-  uint64_t* tempty_bar = bars + 2 * stages + 2;  // leader's copy is live: one arrival per CTA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * stages + 4);
-  uint32_t* abort_s = tmem_slot + 1;
-  const Abort ab{abort_s, abort_flag, spin_limit};
-  const int nkt = num_k_blocks * segs;  // split-bf16: K loop over [A_hi | A_lo | A_hi] x [B_hi | B_hi | B_lo]
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    if (kTmaStore) tma_prefetch_desc(&tmD);
-    if (diag != nullptr && blockIdx.x == 0) {  // SM clock of this launch = d(clock64) / d(globaltimer)
-      unsigned long long g;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
-      diag[0] = clock64();
-      diag[1] = static_cast<long long>(g);
-    }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < stages; ++s) {
-      mbar_init(&full_bar[s], 2);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], 2);
-    }
-    *abort_s = 0;
-    fence_barrier_init();
-  }
-  cluster_sync();
-  if (warp == 2) tmem_alloc_pair(tmem_slot, 512);
-  tc_fence_before();
-  cluster_sync();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int num_tiles = num_m_blocks * num_n_blocks;
-  const int panel_tiles = panel * num_n_blocks;
-  auto decode = [&](int tile, int& m_blk, int& n_blk) {
-    const int p = tile / panel_tiles;
-    const int r = tile - p * panel_tiles;
-    const int m0 = p * panel;
-    const int mcnt = min(panel, num_m_blocks - m0);
-    n_blk = r / mcnt;
-    m_blk = m0 + (r - n_blk * mcnt);
-  };
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = pair; tile < num_tiles && !aborted(ab); tile += num_pairs) {
-        int m_blk, n_blk;
-        decode(tile, m_blk, n_blk);
-        for (int kb = 0; kb < nkt; ++kb) {
-          const int seg = kb / num_k_blocks, r = kb - seg * num_k_blocks;
-          mbar_wait(&empty_bar[stage], phase ^ 1, ab);
-          uint8_t* sa = smem + static_cast<size_t>(stage) * stage_bytes;
-          if (crank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * stage_bytes);
-          else mbar_arrive_remote(&full_bar[stage], 0);
-          tma_load_2d_pair(sa, &tmA, &full_bar[stage], (seg == 1 ? k_pad : 0) + r * kBlockK,
-                           m_blk * 256 + static_cast<int>(crank) * kBlockM, kEvictNormal);
-          tma_load_2d_pair(sa + a_bytes, &tmB, &full_bar[stage], (seg == 2 ? k_pad : 0) + r * kBlockK,
-                           n_blk * bn + static_cast<int>(crank) * (bn / 2), kEvictLast);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (crank == 0 && lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(256, bn);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = pair; tile < num_tiles && !aborted(ab); tile += num_pairs) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1, ab);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(acc * bn);
-        for (int kb = 0; kb < nkt; ++kb) {
-          mbar_wait(&full_bar[stage], phase, ab);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + static_cast<size_t>(stage) * stage_bytes);
-          const uint64_t da = umma_desc_sw128(sa);
-          const uint64_t db = umma_desc_sw128(sa + a_bytes);
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      if (signal && prev >= 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) umma_bf16_pair(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-          umma_commit_pair_mc(&empty_bar[stage], 0x3);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_pair_mc(&tfull_bar[acc], 0x3);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp - 4;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    [[maybe_unused]] int sub = 0;
-    for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-      int m_blk, n_blk;
-      decode(tile, m_blk, n_blk);
-      mbar_wait(&tfull_bar[acc], acc_phase, ab);
-      tc_fence_after();
-      const int row = m_blk * 256 + static_cast<int>(crank) * kBlockM + q * 32 + lane;
-      const bool row_ok = row < m_store;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * bn);
-      if (kTmaStore) {
-        // Epilogue through shared memory + cp.async.bulk.tensor stores: whole 128-byte lines leave the SM, so the L2
-        // never holds partially written lines (the direct 32-byte stores of round 1 made it fetch them from DRAM:
-        // dram reads ~ bytes written).  Sub-tiles of 64 columns; two staging buffers; thread 128 owns the bulk group.
-        const int r_in = q * 32 + lane;                       // row inside this CTA's 128-row half
-        const int row0 = m_blk * 256 + static_cast<int>(crank) * kBlockM;
-        for (int c0 = 0; c0 < bn; c0 += 64, ++sub) {
-          uint8_t* buf = out_stage + (sub & 1) * kOutTileBytes;
-          if (threadIdx.x == 128) bulk_wait_group_read<1>();  // the store that last read this buffer has drained it
-          named_bar_sync(2, 128);
-          const int ncols = min(64, bn - c0);
+      for (int hr = 0; hr < 2; ++hr) {
+        const int row = m_blk * kBlockM + rbase + 8 * hr;
+        if (row >= m_store) continue;
+        OutT* drow = D + static_cast<long long>(row) * ldd;
 #pragma unroll
-          for (int cc = 0; cc < 64; cc += 16) {
-            if (cc < ncols) {
-              uint32_t r[16];
-              tmem_ld16(taddr + c0 + cc, r);
-              tmem_ld_wait();
-              const int n = n_blk * bn + c0 + cc;
-              uint32_t w[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                float x0 = __uint_as_float(r[2 * j]), x1 = __uint_as_float(r[2 * j + 1]);
-                if (bias != nullptr) { x0 += __ldg(bias + n + 2 * j); x1 += __ldg(bias + n + 2 * j + 1); }
-                if (ACT == 1) { x0 = fmaxf(x0, 0.0f); x1 = fmaxf(x1, 0.0f); }
-                if (ACT == 2) { x0 = sigmoid_acc(x0); x1 = sigmoid_acc(x1); }
-                if constexpr (std::is_same<OutT, __half>::value) w[j] = pack_f16x2(x0, x1);
-                else w[j] = pack_bf16x2(x0, x1);
-              }
-              // 128B swizzle: 16-byte chunk j of row r sits at position j ^ (r & 7)
-              const int j0 = cc >> 3;
-              const uint32_t base = smem_u32(buf) + static_cast<uint32_t>(r_in) * 128u;
-              sts_v4(base + (static_cast<uint32_t>((j0) ^ (r_in & 7)) << 4), w[0], w[1], w[2], w[3]);
-              sts_v4(base + (static_cast<uint32_t>((j0 + 1) ^ (r_in & 7)) << 4), w[4], w[5], w[6], w[7]);
+        for (int jg = 0; jg < kBlockN / 8; ++jg) {
+          const int n = n_blk * kBlockN + 8 * jg + 2 * q;
+          if (n < n_store) {
+            float x0 = d[4 * jg + 2 * hr], x1 = d[4 * jg + 2 * hr + 1];
+            if (bias != nullptr) {
+              const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + n));
+              x0 += b2.x;
+              x1 += b2.y;
+            }
+            if (ACT == 1) { x0 = fmaxf(x0, 0.0f); x1 = fmaxf(x1, 0.0f); }
+            if (ACT == 2) { x0 = sigmoid_acc(x0); x1 = sigmoid_acc(x1); }
+            if constexpr (sizeof(OutT) == 4) {
+              *reinterpret_cast<float2*>(drow + n) = make_float2(x0, x1);
+            } else if constexpr (std::is_same<OutT, __half>::value) {
+              *reinterpret_cast<uint32_t*>(drow + n) = pack_f16x2(x0, x1);
+            } else {
+              *reinterpret_cast<uint32_t*>(drow + n) = pack_bf16x2(x0, x1);
             }
           }
-          fence_proxy_async_smem();                           // generic-proxy writes -> visible to the TMA store
-          named_bar_sync(2, 128);
-          if (threadIdx.x == 128) {
-            tma_store_2d_hint(&tmD, buf, n_blk * bn + c0, row0, kEvictFirst);   // clipped by the tensor map
-            bulk_commit_group();
-          }
-        }
-      } else {
-      OutT* drow = D + static_cast<long long>(row) * ldd;
-      for (int c = 0; c < bn; c += 16) {
-        uint32_t r[16];
-        tmem_ld16(taddr + c, r);
-        tmem_ld_wait();
-        const int n = n_blk * bn + c;
-        if (row_ok && n < n_store) {
-          float v[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float x = __uint_as_float(r[j]);
-            if (bias != nullptr) x += __ldg(bias + n + j);
-            if (ACT == 1) x = fmaxf(x, 0.0f);
-            if (ACT == 2) x = sigmoid_acc(x);
-            v[j] = x;
-          }
-          if constexpr (sizeof(OutT) == 4) {
-#pragma unroll
-            for (int j = 0; j < 2; ++j)
-              st_global_v8(drow + n + 8 * j, __float_as_uint(v[8 * j]), __float_as_uint(v[8 * j + 1]),
-                           __float_as_uint(v[8 * j + 2]), __float_as_uint(v[8 * j + 3]), __float_as_uint(v[8 * j + 4]),
-                           __float_as_uint(v[8 * j + 5]), __float_as_uint(v[8 * j + 6]), __float_as_uint(v[8 * j + 7]));
-          } else if constexpr (std::is_same<OutT, __half>::value) {
-            st_global_v8(drow + n, pack_f16x2(v[0], v[1]), pack_f16x2(v[2], v[3]), pack_f16x2(v[4], v[5]),
-                         pack_f16x2(v[6], v[7]), pack_f16x2(v[8], v[9]), pack_f16x2(v[10], v[11]),
-                         pack_f16x2(v[12], v[13]), pack_f16x2(v[14], v[15]));
-          } else {
-            st_global_v8(drow + n, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
-                         pack_bf16x2(v[6], v[7]), pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]),
-                         pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
-          }
         }
       }
-      }
-      // this CTA's 128 epilogue threads are done with accumulator `acc`: one arrival per CTA at the leader
-      tc_fence_before();
-      named_bar_sync(2, 128);
-      if (threadIdx.x == 128) {
-        if (crank == 0) mbar_arrive(&tempty_bar[acc]);
-        else mbar_arrive_remote(&tempty_bar[acc], 0);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-    if (kTmaStore && threadIdx.x == 128) bulk_wait_group<0>();  // all stores complete before the CTA may exit
   }
 
   __syncwarp();
-  tc_fence_before();
-  cluster_sync();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
-  }
-  if (diag != nullptr && threadIdx.x == 0 && blockIdx.x == 0) {
+  if (diag != nullptr && threadIdx.x == 128 && blockIdx.x == 0) {
     unsigned long long g;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
     diag[2] = clock64();
@@ -461,15 +181,11 @@ gemm_bf16_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 
 }  // namespace
 
-size_t gemm_smem_bytes(int bn, int stages) {
-  return 1024 + static_cast<size_t>(stages) * (kBlockM * kBlockK * 2 + bn * kBlockK * 2) + (2 * stages + 4) * 8 + 32;
-}
-
 // Launch.  a: [m_pad rows, k_pad] bf16 (m_pad % 128 == 0, k_pad % 64 == 0); b: [n_pad rows, k_pad] bf16 with
 // n_pad % bn == 0.  Writes D rows < m_store and columns < n_store (n_store % 16 == 0).
 cudaError_t launch_gemm_bf16(const GemmArgs& g, cudaStream_t stream) {
   if (g.m_pad % kBlockM || g.k_pad % kBlockK || g.bn % 16 || g.bn < 16 || g.bn > 256 || g.n_pad % g.bn ||
-      g.n_store % 16)
+      g.n_store % 16 || g.ldd % 2)
     return cudaErrorInvalidValue;
   CUtensorMap tmA, tmB;
   const int segs = g.segs == 3 ? 3 : 1;
@@ -477,83 +193,19 @@ cudaError_t launch_gemm_bf16(const GemmArgs& g, cudaStream_t stream) {
   const long long spin_limit = g.spin_limit > 0 ? g.spin_limit : kSpinLimitDefault;
   cudaError_t e = make_tmap_bf16_2d(&tmA, g.a, k_inner, g.m_pad, g.lda, kBlockK, kBlockM);
   if (e != cudaSuccess) return e;
-  e = make_tmap_bf16_2d(&tmB, g.b, k_inner, g.n_pad, g.ldb, kBlockK, g.bn);
+  e = make_tmap_bf16_2d(&tmB, g.b, k_inner, g.n_pad, g.ldb, kBlockK, kBlockN);
   if (e != cudaSuccess) return e;
 
-  const char* pair_env = getenv("IE_GEMM_PAIR");   // IE_GEMM_PAIR=0: single-CTA kernel (development knob)
-  const int use_pair = pair_env ? atoi(pair_env) : 1;
-  const int sms0 = g.num_sms > 0 ? g.num_sms : 148;
-  if (use_pair && g.m_pad % 256 == 0 && g.bn % 16 == 0 && (g.m_pad / 256) * (g.n_pad / g.bn) >= sms0 / 2) {
-    // CTA-pair path: M = 256 tiles
-    CUtensorMap tmBh;
-    e = make_tmap_bf16_2d(&tmBh, g.b, k_inner, g.n_pad, g.ldb, kBlockK, g.bn / 2);
-    if (e != cudaSuccess) return e;
-    int stages = 8;
-    const char* tma_env = getenv("IE_GEMM_TMA_STORE");            // IE_GEMM_TMA_STORE=0: direct 256-bit stores (A/B runs)
-    // 16-bit outputs: SMEM + TMA stores.  The store box is 64 columns wide: N tiles that are not a multiple of 64 would
-    // let a tile's last box cover its neighbour's columns, so those keep the direct stores (unless there is one N tile
-    // and the tensor map clips the box)
-    const bool tma_store = g.out_bf16 != 0 && !(tma_env && atoi(tma_env) == 0) && (g.bn % 64 == 0 || g.n_pad == g.bn);
-    auto pair_smem = [&](int st) {
-      return 1024 + static_cast<size_t>(st) * (kBlockM * kBlockK * 2 + (g.bn / 2) * kBlockK * 2) +
-             (tma_store ? 2 * 128 * 128 : 0) + (2 * st + 4) * 8 + 32;
-    };
-    CUtensorMap tmD = tmA;                                        // placeholder for the f32-output instantiations
-    if (tma_store) {
-      if (g.ldd % 8 || g.n_store % 8) return cudaErrorInvalidValue;
-      e = make_tmap_bf16_2d(&tmD, g.d, static_cast<uint64_t>(g.n_store), static_cast<uint64_t>(g.m_store), g.ldd, 64, 128);
-      if (e != cudaSuccess) return e;
-    }
-    while (stages > 2 && pair_smem(stages) > 227 * 1024) --stages;
-    const size_t smem = pair_smem(stages);
-    const int num_m_blocks = g.m_pad / 256;
-    const int num_n_blocks = g.n_pad / g.bn;
-    const int num_k_blocks = g.k_pad / kBlockK;
-    const int grid = 2 * (sms0 / 2);
-    // m-blocks per panel (tile order: m fastest inside a panel, then n).  The CTA pairs running together then share
-    // ~panel A blocks and ~num_pairs/panel B tiles: with 8 the working set is ~10 MB of A + ~12 MB of B, far inside the
-    // L2 even next to the output stream (round 1's 37 kept 93 MB live: ncu showed 40 GB of DRAM reads for 3.3 GB of
-    // operands in a 2400 x 9600 projection -- profiles/README.md)
-    int panel = 8;
-    if (const char* v = getenv("IE_GEMM_PANEL")) panel = atoi(v);
-    if (panel < 1) panel = 1;
-#define IE_LAUNCH_PAIR(OUT, ACT)                                                                                  \
-  do {                                                                                                            \
-    auto kfn = gemm_bf16_pair_kernel<OUT, ACT>;                                                                   \
-    e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));           \
-    if (e != cudaSuccess) return e;                                                                               \
-    kfn<<<grid, kGemmThreads, smem, stream>>>(tmA, tmBh, tmD, reinterpret_cast<OUT*>(g.d), g.bias, g.m_store,     \
-                                              g.n_store, g.ldd, num_m_blocks, num_n_blocks, num_k_blocks, g.bn,   \
-                                              stages, panel, segs, g.k_pad, g.abort_flag, spin_limit, g.diag,     \
-                                              tma_store ? 1 : 0);                                                 \
-  } while (0)
-    if (g.out_bf16 == 2) {
-      if (g.act != 0) return cudaErrorInvalidValue;
-      IE_LAUNCH_PAIR(__half, 0);
-    } else if (g.out_bf16) {
-      if (g.act == 0) IE_LAUNCH_PAIR(__nv_bfloat16, 0);
-      else if (g.act == 1) IE_LAUNCH_PAIR(__nv_bfloat16, 1);
-      else IE_LAUNCH_PAIR(__nv_bfloat16, 2);
-    } else {
-      if (g.act == 0) IE_LAUNCH_PAIR(float, 0);
-      else if (g.act == 1) IE_LAUNCH_PAIR(float, 1);
-      else IE_LAUNCH_PAIR(float, 2);
-    }
-#undef IE_LAUNCH_PAIR
-    return cudaGetLastError();
-  }
-
-  int stages = 6;
-  while (stages > 2 && gemm_smem_bytes(g.bn, stages) > 227 * 1024) --stages;
-  const size_t smem = gemm_smem_bytes(g.bn, stages);
+  const size_t smem = 1024 + static_cast<size_t>(kGemmStages) * kGemmStageBytes + 2 * kGemmStages * 8 + 32;
   const int num_m_blocks = g.m_pad / kBlockM;
-  const int num_n_blocks = g.n_pad / g.bn;
+  const int num_n_blocks = (g.n_pad + kBlockN - 1) / kBlockN;
   const int num_k_blocks = g.k_pad / kBlockK;
   const int num_tiles = num_m_blocks * num_n_blocks;
-  const int sms = g.num_sms > 0 ? g.num_sms : 148;
+  const int sms = g.num_sms > 0 ? g.num_sms : 132;
   const int grid = num_tiles < sms ? num_tiles : sms;
-  int panel = sms / 2;
-  if (panel < 1) panel = 1;
+  // m-blocks per panel (tile order: m fastest inside a panel, then n): the CTAs running together share ~16 A blocks
+  // (4 MB at K = 1024) and ~grid/16 B tiles, far inside the 50 MB L2 next to the output stream
+  const int panel = 16;
 
 #define IE_LAUNCH(OUT, ACT)                                                                                        \
   do {                                                                                                             \
@@ -561,8 +213,8 @@ cudaError_t launch_gemm_bf16(const GemmArgs& g, cudaStream_t stream) {
     e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));            \
     if (e != cudaSuccess) return e;                                                                                \
     kfn<<<grid, kGemmThreads, smem, stream>>>(tmA, tmB, reinterpret_cast<OUT*>(g.d), g.bias, g.m_store, g.n_store, \
-                                              g.ldd, num_m_blocks, num_n_blocks, num_k_blocks, g.bn, stages, panel,  \
-                                              segs, g.k_pad, g.abort_flag, spin_limit, g.diag);                    \
+                                              g.ldd, num_m_blocks, num_n_blocks, num_k_blocks, panel, segs,        \
+                                              g.k_pad, g.abort_flag, spin_limit, g.diag);                          \
   } while (0)
 
   if (g.out_bf16 == 2) {

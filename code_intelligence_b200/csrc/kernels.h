@@ -1,4 +1,4 @@
-// Internal launch interfaces between the C-ABI layer (api.cu) and the sm_100a kernels.
+// Internal launch interfaces between the C-ABI layer (api.cu) and the sm_90a kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -23,7 +23,7 @@ struct GemmArgs {
   int m_pad, n_pad, k_pad;
   long long lda, ldb, ldd;
   int m_store, n_store;
-  int bn;        // N tile (multiple of 16, <= 256, divides n_pad)
+  int bn;        // padding granularity of N (multiple of 16, <= 256, divides n_pad); the kernel's N tile is 256
   int act;       // 0 none, 1 relu, 2 sigmoid
   int out_bf16;  // output type: 0 f32, 1 bf16, 2 fp16 (act must be 0)
   int num_sms;
@@ -34,56 +34,36 @@ struct GemmArgs {
 };
 cudaError_t launch_gemm_bf16(const GemmArgs& g, cudaStream_t stream);
 
-// ---- fallback recurrent step (lstm.cu): one timestep of one 256-row batch per launch -------------------------------
-struct LstmStepArgs {
-  CUtensorMap tm_h;  // hidden-state ring of the time chunk [(Tc+1)*b_pad rows, ring cols], box {64, 128}
-  CUtensorMap tm_w;  // W_hh [4*out_pad rows, cols], box {64, 128}; rows ordered [slice][unit][gate], 32 units / slice
-  const void* gx;    // f32 or bf16 [rows, 4*out_pad] (bias folded in): row t*b_pad + brow of the chunk, or token id
-  const int* tok;    // optional time-major token ids of the whole call (per-token input-projection table)
-  float* c;          // [b_pad, out_pad] cell state
-  __nv_bfloat16* y;  // ring (slot 0 = h before the chunk (zeros at t0 = 0); slot t+1 = h_t, t chunk-local)
-  float* raw;        // optional [b_pad, T_total, raw_ld] f32 copy of h (get_raw_features)
-  float* pool_sum;   // optional [b_pad, out_pad] (last layer only; formats: lstm_common.cuh)
-  float* pool_max;
-  float* pool_last;
-  const int* lengths;  // [b_pad]
-  unsigned* abort_flag;
-  long long spin_limit;
-  int t, t0, T_total;  // chunk-local timestep, global index of the chunk's first timestep, timesteps of the call
-  int b_pad;           // rows per time slot (multiple of 256)
-  int g;               // which 256-row batch of the slot
-  int u, n_cta, out_pad, kh_pad;
-  long long ldy, raw_ld;
-  int gate_mode, gx_bf16, segs;
-};
-cudaError_t launch_lstm_step(const LstmStepArgs& a, cudaStream_t stream);
-
-// ---- persistent recurrent layer (lstm_layer.cu): all timesteps of a layer (or of a time chunk) in one cooperative launch,
-//      up to kMaxBatches batches of 256 rows; (timestep, batch, tile) items dealt round-robin over all CTA pairs
+// ---- recurrent layer (lstm_layer.cu): all timesteps of a layer (or of a time chunk) in one cooperative launch, up to
+//      kMaxBatches batches of 256 rows; (timestep, batch, row half, tile) items dealt round-robin over all CTAs.  With
+//      single_step the same kernel runs one timestep per launch (the fallback when the grid cannot be co-resident).
 constexpr int kMaxBatches = 12;
 struct LstmLayerArgs {
-  CUtensorMap tm_h, tm_w;  // as LstmStepArgs
-  CUtensorMap tm_h64;      // same tensor as tm_h with box {64, 64}: the quarter tile one CTA multicasts (mc != 0)
+  CUtensorMap tm_h;        // hidden-state ring of the time chunk [(Tc+1)*b_pad rows, ring cols], box {64, 128}
+  CUtensorMap tm_w;        // W_hh [4*out_pad rows, cols], box {64, 256}; rows ordered as api.cu slice_perm
+  CUtensorMap tm_h64;      // same tensor as tm_h with box {64, 64}: the half tile one CTA multicasts (mc != 0)
   CUtensorMap tm_x;        // pre_nkb > 0: the PREVIOUS layer's ring (slot t+1 = this layer's x_t), box {64, 128}
   int pre_nkb;             // > 0: fuse the input projection into the K loop -- pre_nkb = kin_pad / 64 k-blocks of
                            // x_t W_ih^T precede the recurrent ones; tm_w then covers [W_ih | W_hh] (inner kin_pad + kh_pad),
                            // gx is unused and `bias` (b_ih + b_hh, permuted like the weight rows) is added instead
   const float* bias;
-  int mc;                  // 1: clusters of two CTA pairs share every h tile by TMA multicast (needs an even number of tiles)
-  int mc_pairs;            // CTA pairs that can be co-resident in clusters of four (lstm_layer_max_pairs() of a check_only query)
-  const void* gx;
-  const int* tok;
-  float* c;
-  __nv_bfloat16* y;
-  float* raw;
-  float* pool_sum;
+  int mc;                  // 1: clusters of two CTAs share every h tile by TMA multicast (needs an even number of tiles)
+  int mc_ctas;             // CTAs that can be co-resident in clusters of two (lstm_layer_max_ctas() of a check_only query)
+  const void* gx;          // f16 or f32 [rows, 4*out_pad] (bias folded in): row t*b_pad + brow of the chunk, or token id
+  const int* tok;          // optional time-major token ids of the whole call (per-token input-projection table)
+  float* c;                // [b_pad, out_pad] cell state
+  __nv_bfloat16* y;        // ring (slot 0 = h before the chunk (zeros at t0 = 0); slot t+1 = h_t, t chunk-local)
+  float* raw;              // optional [b_pad, T_total, raw_ld] f32 copy of h (get_raw_features)
+  float* pool_sum;         // optional [b_pad, out_pad] (last layer only; formats: lstm_common.cuh)
   float* pool_max;
   float* pool_last;
-  const int* lengths;
+  const int* lengths;      // [b_pad]
   unsigned* step_done;   // [T*ng] zero-initialised (step, batch) counters of this launch
   unsigned* abort_flag;
   long long spin_limit;
   int T, t0, T_total;    // timesteps in this launch, global index of the first, timesteps of the whole call
+  int single_step;       // 1: only chunk-local timestep t_step, one item per CTA, no counters, not cooperative
+  int t_step;
   int ng;                // batches of 256 rows
   int u, n_cta, out_pad, kh_pad;
   long long ldy, raw_ld;
@@ -95,8 +75,8 @@ struct LstmLayerArgs {
   long long* diag;       // optional [4]: {clock64, globaltimer ns} at the start and end of CTA 0 (SM clock of the launch)
 };
 cudaError_t launch_lstm_layer(const LstmLayerArgs& a, cudaStream_t stream);
-int lstm_layer_pairs(const LstmLayerArgs& a);  // CTA pairs the launch will use
-int lstm_layer_max_pairs();                    // result of the last check_only query on this thread
+int lstm_layer_ctas(const LstmLayerArgs& a);  // CTAs the launch will use
+int lstm_layer_max_ctas();                    // result of the last check_only query on this thread
 
 // ---- small memory-bound kernels (misc.cu) --------------------------------------------------------
 // ids [B, T] int64 (batch-first, right padded) -> x0 [(T*b_pad), ldx] bf16, time-major rows t*b_pad + b

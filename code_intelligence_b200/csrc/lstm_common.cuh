@@ -1,6 +1,5 @@
-// Arithmetic shared by the recurrent kernels (lstm_layer.cu = the persistent kernel, lstm.cu = the per-timestep
-// fallback): the LSTM cell update on one 16-column accumulator chunk and the masked concat-pool accumulation.  Both
-// kernels call exactly these functions with the same association of operations, so every path gives the same bits.
+// Arithmetic of the recurrent kernel (lstm_layer.cu; its persistent launch and the per-timestep fallback launch run the
+// same code): the LSTM cell update of one hidden unit and the masked concat-pool accumulation.
 //
 // Reference arithmetic: torch nn.LSTM as wrapped by fastai's AWD_LSTM, called at
 // Issue_Embeddings/flask_app/inference.py:57,68 (gate rows i|f|g|o, c_t = f*c_{t-1} + i*g, h_t = o*tanh(c_t));
@@ -31,77 +30,44 @@ __device__ __forceinline__ float tanh_ieee(float x) {
   return copysignf(t, x);
 }
 
-// One accumulator chunk: 16 TMEM columns = 4 hidden units x (i, f, g, o) of one batch row.
-//   acc : the h_{t-1} W_hh^T part (f32 bits from tcgen05.ld)       gx : x_t W_ih^T + b_ih + b_hh (4 units x 4 gates)
-__device__ __forceinline__ void lstm_cell4(const uint32_t (&acc)[16], const float4 (&gx)[4], const float (&cprev)[4],
-                                           float (&cnew)[4], float (&hn)[4], int gate_mode) {
-#pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    const float zi = __uint_as_float(acc[4 * u + 0]) + gx[u].x;
-    const float zf = __uint_as_float(acc[4 * u + 1]) + gx[u].y;
-    const float zg = __uint_as_float(acc[4 * u + 2]) + gx[u].z;
-    const float zo = __uint_as_float(acc[4 * u + 3]) + gx[u].w;
-    if (gate_mode == kGatesFast) {
-      cnew[u] = sigmoid_fast(zf) * cprev[u] + sigmoid_fast(zi) * tanh_fast(zg);
-      hn[u] = sigmoid_fast(zo) * tanh_fast(cnew[u]);
-    } else if (gate_mode == kGatesExp) {
-      cnew[u] = sigmoid_acc(zf) * cprev[u] + sigmoid_acc(zi) * tanh_acc(zg);
-      hn[u] = sigmoid_acc(zo) * tanh_acc(cnew[u]);
-    } else {
-      cnew[u] = sigmoid_ieee(zf) * cprev[u] + sigmoid_ieee(zi) * tanh_ieee(zg);
-      hn[u] = sigmoid_ieee(zo) * tanh_ieee(cnew[u]);
-    }
-  }
-}
-
-// fp16 x 16 (one 256-bit load) -> the 4 x float4 Gx operands of a chunk.  The hoisted input projections are stored as
-// IEEE half (11-bit significand: 8x finer than bf16 at the same bytes; |Gx| is O(1), far inside the half range)
-__device__ __forceinline__ void gx_unpack_f16(const uint32_t* p, float4 (&gx)[4]) {
-#pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&p[2 * u]));
-    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&p[2 * u + 1]));
-    gx[u] = make_float4(a.x, a.y, b.x, b.y);
+// One hidden unit of one batch row.  z* = the accumulator (h_{t-1} W_hh^T, plus x_t W_ih^T when the input projection
+// rides the K loop) + Gx (x_t W_ih^T + b_ih + b_hh) or the bias; gate order i, f, g, o as in torch.
+__device__ __forceinline__ void lstm_cell1(float zi, float zf, float zg, float zo, float cprev, float& cnew, float& hn,
+                                           int gate_mode) {
+  if (gate_mode == kGatesFast) {
+    cnew = sigmoid_fast(zf) * cprev + sigmoid_fast(zi) * tanh_fast(zg);
+    hn = sigmoid_fast(zo) * tanh_fast(cnew);
+  } else if (gate_mode == kGatesExp) {
+    cnew = sigmoid_acc(zf) * cprev + sigmoid_acc(zi) * tanh_acc(zg);
+    hn = sigmoid_acc(zo) * tanh_acc(cnew);
+  } else {
+    cnew = sigmoid_ieee(zf) * cprev + sigmoid_ieee(zi) * tanh_ieee(zg);
+    hn = sigmoid_ieee(zo) * tanh_ieee(cnew);
   }
 }
 
 // ---- masked concat-pool accumulators in global memory ------------------------------------------------------------
-// pool_sum : f32, sequential sum over t (one add per timestep, in timestep order): an L2 reduction (red.add.v4.f32) --
-//            no load, no latency, no accumulator registers.  The (step, batch) counter protocol of the persistent kernel
-//            orders step t's reduction after step t-1's (gpu-scope fence before the counter increment), so it is the same
+// pool_sum : f32, sequential sum over t (one add per timestep, in timestep order): an L2 reduction (red.add.f32) --
+//            no load, no accumulator registers.  The (step, batch) counter protocol of the persistent kernel orders
+//            step t's reduction after step t-1's (gpu-scope fence before the counter increment), so it is the same
 //            sequential f32 sum a register accumulator would give: identical bits on every path.
-// pool_max : f32 running max; it travels like the cell state (the caller loads the previous value from L2 before the
-//            accumulator is ready and this function stores the new one) -- 16 scalar red.max per thread and item put
-//            ~6 us of L2 atomic traffic on the last layer's step chain.
+// pool_max : f32 running max; it travels like the cell state (read from L2 after the (t-1, batch) counter was seen)
 // pool_last: f32, h at t == len-1
-__device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
-  asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void red_add_f32(float* p, float v) {
+  asm volatile("red.relaxed.gpu.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
 }
-// po: offset of the 4 units in the [row, out_pad] accumulator arrays; mprev: pool_max[po..po+3] (read when 0 < tg < len);
-// tg: global timestep; len: valid length of the row
-__device__ __forceinline__ void pool_accumulate4(float* pool_sum, float* pool_max, float* pool_last, long long po,
-                                                 const float (&hn)[4], const float4& mprev, int tg, int len) {
+// po: offset of the unit in the [row, out_pad] accumulator arrays; tg: global timestep; len: valid length of the row
+__device__ __forceinline__ void pool_accumulate1(float* pool_sum, float* pool_max, float* pool_last, long long po,
+                                                 float hn, int tg, int len) {
   if (tg >= len) return;
-  const float4 h4 = make_float4(hn[0], hn[1], hn[2], hn[3]);
   if (tg == 0) {
-    __stcg(reinterpret_cast<float4*>(pool_sum + po), h4);
-    __stcg(reinterpret_cast<float4*>(pool_max + po), h4);
+    __stcg(pool_sum + po, hn);
+    __stcg(pool_max + po, hn);
   } else {
-    red_add_v4(pool_sum + po, hn[0], hn[1], hn[2], hn[3]);
-    __stcg(reinterpret_cast<float4*>(pool_max + po),
-           make_float4(fmaxf(mprev.x, hn[0]), fmaxf(mprev.y, hn[1]), fmaxf(mprev.z, hn[2]), fmaxf(mprev.w, hn[3])));
+    red_add_f32(pool_sum + po, hn);
+    __stcg(pool_max + po, fmaxf(__ldcg(pool_max + po), hn));
   }
-  if (tg == len - 1) __stcg(reinterpret_cast<float4*>(pool_last + po), h4);
-}
-
-// sum / last part only (the persistent kernel writes the running max of two chunks with one 256-bit store)
-__device__ __forceinline__ void pool_sum_last4(float* pool_sum, float* pool_last, long long po, const float (&hn)[4], int tg,
-                                               int len) {
-  if (tg >= len) return;
-  const float4 h4 = make_float4(hn[0], hn[1], hn[2], hn[3]);
-  if (tg == 0) __stcg(reinterpret_cast<float4*>(pool_sum + po), h4);
-  else red_add_v4(pool_sum + po, hn[0], hn[1], hn[2], hn[3]);
-  if (tg == len - 1) __stcg(reinterpret_cast<float4*>(pool_last + po), h4);
+  if (tg == len - 1) __stcg(pool_last + po, hn);
 }
 
 // order-preserving u32 encoding of f32 (used by pr_curve.cu to sort scores as integers)
@@ -122,15 +88,10 @@ __host__ __device__ __forceinline__ float dec_max(uint32_t e) {
 
 // h_t in the ring: bf16 (hi); with `lo_off` > 0 also the bf16 residual h - hi at column offset lo_off (the split-bf16
 // fp32-accurate mode: h ~ hi + lo to ~16 mantissa bits)
-__device__ __forceinline__ void store_h4(__nv_bfloat16* yp, const float (&hn)[4], long long lo_off) {
-  const __nv_bfloat162 a = __floats2bfloat162_rn(hn[0], hn[1]);
-  const __nv_bfloat162 b = __floats2bfloat162_rn(hn[2], hn[3]);
-  *reinterpret_cast<uint2*>(yp) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
-  if (lo_off > 0) {
-    const float2 fa = __bfloat1622float2(a), fb = __bfloat1622float2(b);
-    *reinterpret_cast<uint2*>(yp + lo_off) =
-        make_uint2(pack_bf16x2(hn[0] - fa.x, hn[1] - fa.y), pack_bf16x2(hn[2] - fb.x, hn[3] - fb.y));
-  }
+__device__ __forceinline__ void store_h1(__nv_bfloat16* yp, float hn, long long lo_off) {
+  const __nv_bfloat16 hi = __float2bfloat16_rn(hn);
+  *yp = hi;
+  if (lo_off > 0) yp[lo_off] = __float2bfloat16_rn(hn - __bfloat162float(hi));
 }
 
 }  // namespace ie

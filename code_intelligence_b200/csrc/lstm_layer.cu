@@ -1,39 +1,37 @@
-// THE persistent recurrent kernel: all timesteps of one LSTM layer (or of one time chunk of it) for up to kMaxBatches
-// independent batches of 256 rows in one launch.  Reference call sites of the arithmetic:
-// Issue_Embeddings/flask_app/inference.py:56-57, :66-68 (reset + forward), pooling :239.
+// THE recurrent kernel: all timesteps of one LSTM layer (or of one time chunk of it) for up to kMaxBatches independent
+// batches of 256 rows in one persistent launch -- or, as the per-timestep fallback, one timestep per launch with the
+// same code.  Reference call sites of the arithmetic: Issue_Embeddings/flask_app/inference.py:56-57, :66-68 (reset +
+// forward), pooling :239.
 //
 //     z_t = Gx[t] + h_{t-1} W_hh^T ; i,f,o = sigmoid ; g = tanh ; c_t = f c_{t-1} + i g ; h_t = o tanh(c_t)
 //
-// Work decomposition ("rotating schedule", round-1 experiment lstm_rot.cu, now the only persistent kernel -- it
-// replaced the static deals of lstm_seq.cu / lstm_wide.cu, which left 23 % of the CTA pairs idle at H = 2400):
-//   * a CTA pair (cluster of 2 on one TPC, tcgen05 cta_group::2) is one M = 256 tensor core: CTA r holds batch rows
-//     [128 r, +128) of the h tile and half of the W_hh tile; an accumulator tile is 256 rows x 256 columns = 64 hidden
-//     units x (i,f,g,o) -- weight rows are pre-permuted to [tile][cta][unit][gate] so a thread finds the four gates of a
-//     unit in adjacent TMEM columns and the cell update needs no cross-thread traffic;
-//   * the work ITEMS  n = t * C + g * tiles + j  (C = ng * tiles; timestep t, batch g, column tile j) are dealt round-robin
-//     in that global order over the P resident pairs: pair p runs items p, p + P, p + 2P, ...  Item n needs h_{t-1} of
-//     batch g, i.e. items n - C - j .. n - C + (tiles - 1 - j), all with smaller indices; every pair walks its items in
-//     increasing order, so the item with the globally smallest index can always run: no wait cycle for any P, C, T.
-//     With C >= 2P + tiles (five batches at H = 2400: 190 >= 148 + 38) an item's inputs were finished two rounds
-//     earlier and every pair issues MMAs back to back;
-//   * per item: K/64 k-blocks of h and W_hh (TMA, 128B swizzle) through ONE 7-stage ring -- two producer threads fill
-//     the halves of a stage independently (weights do not depend on the step, so their producer runs ahead of the h
-//     dependency) -> 4 x tcgen05.mma per k-block into one of two TMEM accumulator slots -> 16 epilogue warps
-//     (tcgen05.ld, + Gx, gates, c_t, h_t as bf16 into slot t+1 of the hidden-state ring = next step's A operand and the
-//     next layer's GEMM input; full 32-byte sectors per store) -> gpu-scope fence + red.add on the (step, batch) counter;
-//   * the cell state moves between SMs from step to step: it lives in global memory (L2) and is read with 256-bit
-//     ld.global.cg (one request per 32-byte sector) after the pair has seen the (t-1, g) counter; on the last layer the
-//     running max of the concat-pool travels the same way and the pooled sum is an L2 reduction (lstm_common.cuh), so
-//     none of them sits on the step's critical path;
-//   * the LAST layer runs the FUSE instantiation: its input projection x_t W_ih^T (38 k-blocks that depend on no step
-//     counter) is accumulated in front of the 13 recurrent k-blocks of every item instead of by a hoisted GEMM -- the
-//     layer's 65 items per timestep cannot fill 74 pairs, and the independent k-blocks hide its step chain (see FUSE);
+// Work decomposition ("rotating schedule"):
+//   * an ITEM is 128 batch rows x one column tile of 256 accumulator columns = 64 hidden units x (i,f,g,o).  Weight rows
+//     are pre-permuted (api.cu slice_perm) so that the wgmma fragment of a thread holds all four gates of a unit: inside
+//     each 16-column chunk, columns 2q, 2q+1 are (i, f) and 8+2q, 9+2q are (g, o) of the chunk's unit q -- the cell update
+//     needs no cross-thread traffic;
+//   * the items  n = t * C + g * 2 tiles + half * tiles + j  (C = ng * 2 tiles; timestep t, batch g, row half, column
+//     tile j) are dealt round-robin in that global order over the P resident CTAs: CTA p runs items p, p + P, ...  Item n
+//     needs h_{t-1} of batch g, i.e. items of step t-1 with smaller indices; every CTA walks its items in increasing
+//     order, so the item with the globally smallest index can always run: no wait cycle for any P, C, T;
+//   * per item: K/64 k-blocks of h and W_hh (TMA, 128B swizzle) through ONE 4-stage ring -- two producer threads fill the
+//     halves of a stage independently (weights do not depend on the step, so their producer runs ahead of the h
+//     dependency) -> two consumer warpgroups (64 rows each) issue 4 x wgmma m64n256k16 per k-block into registers and
+//     then run the epilogue (+ Gx, gates, c_t, h_t as bf16 into slot t+1 of the hidden-state ring = next step's A operand
+//     and the next layer's GEMM input) -> gpu-scope fence + red.add on the (step, batch) counter;
+//   * the cell state moves between SMs from step to step: it lives in global memory (L2), read with ld.global.cg after
+//     the CTA has seen the (t-1, g) counter; on the last layer the running max of the concat-pool travels the same way
+//     and the pooled sum is an L2 reduction (lstm_common.cuh);
+//   * the LAST layer runs the FUSE instantiation: its input projection x_t W_ih^T (k-blocks that depend on no step counter)
+//     is accumulated in front of the recurrent k-blocks of every item instead of by a hoisted GEMM (see FUSE);
 //   * split-bf16 ("fp32-accurate") mode: segs = 3 runs the K loop over [h_hi | h_lo | h_hi] x [W_hi | W_hi | W_lo]
 //     (hi = bf16(x), lo = bf16(x - hi); the dropped lo*lo term is 2^-18 relative) -- same kernel, three times the MMAs.
 //
-// All CTAs must be co-resident: the launch is cooperative (cudaLaunchAttributeCooperative), so it either gets the
-// whole grid resident or fails; a wait that still exceeds its limit raises the abort protocol of ptx.cuh (no trap).
+// All CTAs of a persistent launch must be co-resident: the launch is cooperative (cudaLaunchAttributeCooperative), so it
+// either gets the whole grid resident or fails; a wait that still exceeds its limit raises the abort protocol of ptx.cuh.
 #include <cmath>
+
+#include <cuda_fp16.h>
 
 #include "kernels.h"
 #include "lstm_common.cuh"
@@ -43,10 +41,13 @@ namespace ie {
 
 namespace {
 
-constexpr int kLThreads = 640;          // 4 role warps + 16 epilogue warps (4 per TMEM lane quarter, 64 columns each)
-constexpr int kLStages = 7;             // operand ring: 7 stages x (h k-block 16 KB + W_hh k-block 16 KB) per CTA
-constexpr int kLTileN = 256;            // accumulator columns per tile = 64 hidden units
-constexpr int kLHalfRows = 128;         // W rows each CTA of the pair contributes
+constexpr int kLThreads = 384;          // warpgroup 0: producers + counter watcher; warpgroups 1, 2: MMA + epilogue
+constexpr int kLStages = 4;             // operand ring: 4 stages x (h k-block 16 KB + W k-block 32 KB)
+constexpr int kLTileN = 256;            // accumulator columns per item = 64 hidden units
+constexpr int kLRows = 128;             // batch rows per item
+constexpr uint32_t kHBytes = kLRows * 64 * 2;
+constexpr uint32_t kWBytes = kLTileN * 64 * 2;
+constexpr uint32_t kStageBytes = kHBytes + kWBytes;
 
 __device__ __forceinline__ void st_release_cta(uint32_t* p, uint32_t v) {
   asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
@@ -69,7 +70,7 @@ __device__ __forceinline__ void wait_seq_ge(const uint32_t* p, uint32_t target, 
 }
 
 struct KArgs {
-  const void* gx;        // f32 or bf16 [rows, 4*out_pad]; row = t_local*b_pad + brow, or the token id (TOK)
+  const void* gx;        // f16 or f32 [rows, 4*out_pad]; row = t_local*b_pad + brow, or the token id (TOK)
   const int* tok;        // TOK: time-major token ids of the whole call, index (t0 + t)*b_pad + brow
   const float* bias;     // FUSE: b_ih + b_hh in the permuted column order (takes the place of Gx)
   float* cstate;         // [b_pad, out_pad]
@@ -79,36 +80,30 @@ struct KArgs {
   float* pool_max;
   float* pool_last;
   const int* lengths;
-  unsigned* step_done;   // [T*ng] zero-initialised (chunk-local)
+  unsigned* step_done;   // [T*ng] zero-initialised (step, batch) counters (nullptr: one timestep per launch)
   unsigned* abort_flag;
   long long spin_limit;
   long long ldy, raw_ld;
   long long* trace;
   long long* diag;
-  int T, t0, T_total, ng, tiles, out_pad, nkb, segs, kh_pad, gate_mode, trace_items, fault;
+  int T, t_begin, t0, T_total, ng, tiles, out_pad, nkb, segs, kh_pad, gate_mode, trace_items, fault;
   int pre_nkb;           // FUSE: k-blocks of the input projection that precede the recurrent ones in every item
 };
 
 // TOK: Gx rows are rows of the per-token input-projection table; GXBF: Gx / table stored as fp16 (f32 otherwise);
 // POOL: last layer -- the masked concat-pool accumulators ride the epilogue;
-// MC: clusters of FOUR CTAs = two sibling pairs (2q, 2q+1).  Sibling pairs always hold items n, n+1 = the same
-//     (timestep, batch) and adjacent column tiles (tiles, C and P even), i.e. they need the SAME h tile: each CTA loads a
-//     quarter of it and multicasts it to its counterpart in the sibling pair, so an h tile leaves the L2 once per two
-//     items.  The kernel is bound by L2 -> SM bytes (both operands stream from L2 at ~9.5 TB/s chip-wide, the practical
-//     LTS limit -- profiles/README.md); this removes a quarter of them.  A stage is refilled only when BOTH pairs have
-//     consumed it (empty barriers count two commits, each multicast to all four CTAs).
+// MC: clusters of TWO CTAs that always hold items n, n+1 (n even) = the same (timestep, batch, row half) and adjacent
+//     column tiles (tiles, C and P even), i.e. they need the SAME h tile: each CTA loads half of it and multicasts it
+//     to both, so an h tile leaves the L2 once per two items.  A stage is refilled only when the consumers of BOTH CTAs
+//     have released it (empty barriers count four arrivals).
 // FUSE: the layer's input projection rides the recurrent K loop instead of a hoisted GEMM + Gx round trip: every item
 //     first accumulates x_t W_ih^T -- pre_nkb k-blocks whose A operand is slot t+1 of the PREVIOUS layer's ring (tm_x)
 //     and whose B operand is the W_ih part of the concatenated weights [W_ih | W_hh] (tm_w) -- and then, once the
 //     (t-1, g) counter has been seen, the nkb k-blocks of h_{t-1} W_hh^T into the same accumulator; the epilogue adds
-//     the bias (f32) where the other instantiations add Gx.  Used for the 800-wide last layer, whose 13 tiles x 5
-//     batches cannot fill 74 pairs: its step chain (MMAs 7.5 us + epilogue + publish + counter + first tile ~ 20 us per
-//     timestep) left the tensor pipe idle 80 % of the time, and the independent W_ih k-blocks now run inside that wait
-//     (the dependency of item k resolves while the pair issues the 38 input-projection k-blocks of item k).  The sum
+//     the bias (f32) where the other instantiations add Gx.  Used for the narrow last layer, whose few items per
+//     timestep leave most CTAs waiting on the step chain: the independent W_ih k-blocks run inside that wait.  The sum
 //     W_ih x + W_hh h + b stays in f32 (no fp16 rounding of Gx), so the fused layer is slightly MORE accurate than the
-//     hoisted form, but its bits differ from the fallback kernel's (tests compare those two with IE_FUSE_LAST=0).
-// The body is shared by two __global__ wrappers below: the production kernel with compile-time clusters of two, and
-// the multicast variant whose clusters of four come from the launch attribute.
+//     hoisted form, but its bits differ from the hoisted form's (tests compare those two with IE_FUSE_LAST=0).
 template <bool TOK, bool GXBF, bool POOL, bool MC, bool FUSE>
 __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const CUtensorMap& tm_w,
                                                 const CUtensorMap& tm_h64, const CUtensorMap& tm_x, const KArgs& a) {
@@ -116,48 +111,38 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
   const uint32_t rawaddr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (rawaddr & 1023u)) & 1023u);
 
-  constexpr uint32_t a_bytes = 128 * 64 * 2;
-  constexpr uint32_t w_bytes = kLHalfRows * 64 * 2;
-  constexpr uint32_t stage_bytes = a_bytes + w_bytes;
-  // ONE ring for both operands (like the GEMM main loop): stage s holds the k-block's h tile and W_hh tile.  The two
-  // producers fill their halves independently -- W_hh does not depend on the step, so its producer runs ahead of the h
-  // dependency -- and the MMA thread waits on one barrier and commits once per k-block.  (Round 1's two 3 x 2-k-block
-  // rings left ~18 % of the MMA thread's time in stage waits: a stage was only refilled after both of its k-blocks.)
   uint8_t* ring = smem;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + kLStages * stage_bytes);
-  uint64_t* full = bars;                    // [kLStages] leader's copy is live: 4 arrivals (h / W producer of each CTA)
-  uint64_t* empty = full + kLStages;        // [kLStages] per CTA: the leader's multicast commit
-  uint64_t* tfull = empty + kLStages;       // [2] accumulator slot holds a finished item (both CTAs' copies live)
-  uint64_t* tempty = tfull + 2;             // [2] accumulator slot drained by both CTAs (leader's copy is live)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  uint32_t* cready = tmem_slot + 1;         // number of this CTA's items whose (t-1, g) counter the watcher has seen
-  uint32_t* abort_s = tmem_slot + 2;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + kLStages * kStageBytes);  // [kLStages] 2 arrivals + bytes
+  uint64_t* empty = full + kLStages;                                             // [kLStages] consumer releases
+  uint32_t* cready = reinterpret_cast<uint32_t*>(empty + kLStages);  // items whose (t-1, g) counter the watcher has seen
+  uint32_t* abort_s = cready + 1;
   const Abort ab{abort_s, a.abort_flag, a.spin_limit};
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   long long* const trace = a.trace;
-  // optional timeline of the pair's first `trace_items` items: [cta][k][12] (%globaltimer ns; slots 8-11 SM cycles)
+  // optional timeline of the CTA's first `trace_items` items: [cta][k][12] (%globaltimer ns)
 #define IE_TRACE(slot, kk) do { if (trace && (kk) < a.trace_items) { unsigned long long _g; \
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(_g)); \
     trace[(static_cast<long long>(blockIdx.x) * a.trace_items + (kk)) * 12 + (slot)] = static_cast<long long>(_g); } } while (0)
-#define IE_TRACE_VAL(slot, kk, v) do { if (trace && (kk) < a.trace_items) \
-    trace[(static_cast<long long>(blockIdx.x) * a.trace_items + (kk)) * 12 + (slot)] = (v); } while (0)
-  const uint32_t crank4 = cluster_ctarank();       // rank in the cluster (0..1, or 0..3 with MC)
-  const uint32_t crank = crank4 & 1u;              // rank in the CTA pair: 0 = leader
-  const uint32_t cpair = crank4 >> 1;              // which pair of the cluster (MC only; 0 otherwise)
-  const uint32_t leader = crank4 & ~1u;            // cluster rank of this pair's leader
-  const uint16_t pmask = static_cast<uint16_t>(0x3u << (2 * cpair));   // the CTAs of this pair
-  const uint16_t emask = MC ? 0xF : pmask;         // who must see a stage release
-  const int pair = blockIdx.x >> 1;
-  const int P = static_cast<int>(gridDim.x >> 1);
+  const uint32_t crank = MC ? cluster_ctarank() : 0u;
+  const int P = static_cast<int>(gridDim.x);
   const int tiles = a.tiles, ng = a.ng;
-  const int C = ng * tiles;
+  const int per_batch = 2 * tiles;                 // items of one (step, batch)
+  const int C = ng * per_batch;
   const long long total = static_cast<long long>(a.T) * C;
   const int b_pad = 256 * ng;
-  const unsigned batch_ctas = 2u * static_cast<unsigned>(tiles);  // CTAs that publish a (step, batch)
-  const int nkt = a.nkb * a.segs;                                   // recurrent k-blocks per item
-  const int pre = FUSE ? a.pre_nkb : 0;                             // input-projection k-blocks per item (before them)
+  const int nkt = a.nkb * a.segs;                  // recurrent k-blocks per item
+  const int pre = FUSE ? a.pre_nkb : 0;            // input-projection k-blocks per item (before them)
+  auto decode = [&](long long n, int& t, int& g, int& half, int& j) {
+    const long long s = n / C;
+    const int c = static_cast<int>(n - s * C);
+    t = a.t_begin + static_cast<int>(s);
+    g = c / per_batch;
+    const int r = c - g * per_batch;
+    half = r / tiles;
+    j = r - half * tiles;
+  };
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tm_h);
@@ -173,282 +158,184 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < kLStages; ++s) {
-      mbar_init(&full[s], 4);
-      mbar_init(&empty[s], MC ? 2 : 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], 2);
+      mbar_init(&full[s], 2);
+      mbar_init(&empty[s], MC ? 4 : 2);
     }
     *cready = 0;
     *abort_s = 0;
     fence_barrier_init();
   }
-  cluster_sync();
-  if (warp == 2) tmem_alloc_pair(tmem_slot, 512);
-  tc_fence_before();
-  cluster_sync();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (MC) cluster_sync();
+  else __syncthreads();
 
-  if (warp == 0) {
-    // ---------------- h producer ------------------------------------------------------------------------------
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
+      // ---------------- h producer ------------------------------------------------------------------------------
       int stage = 0;
       uint32_t phase = 0;
       int k = 0;
-      for (long long n = pair; n < total && !aborted(ab); n += P, ++k) {
-        const int t = static_cast<int>(n / C);
-        const int g = static_cast<int>(n - static_cast<long long>(t) * C) / tiles;
-        const int row0 = t * b_pad + g * 256 + static_cast<int>(crank) * 128;  // ring slot t = h_{t-1} (chunk-local)
+      for (long long n = blockIdx.x; n < total && !aborted(ab); n += P, ++k) {
+        int t, g, half, j;
+        decode(n, t, g, half, j);
+        const int row0 = t * b_pad + g * 256 + half * kLRows;   // ring slot t = h_{t-1} (chunk-local)
         if constexpr (FUSE) {
           // x_t = slot t+1 of the previous layer's ring (complete before this launch): no dependency on the step counters
           for (int kb = 0; kb < pre; ++kb) {
             mbar_wait(&empty[stage], phase ^ 1, ab);
-            if (crank == 0) mbar_arrive_expect_tx(&full[stage], 2 * a_bytes);
-            else mbar_arrive_remote(&full[stage], leader);
-            tma_load_2d_pair(ring + stage * stage_bytes, &tm_x, &full[stage], kb * 64, row0 + b_pad, kEvictNormal);
+            mbar_arrive_expect_tx(&full[stage], kHBytes);
+            tma_load_2d(ring + stage * kStageBytes, &tm_x, &full[stage], kb * 64, row0 + b_pad, kEvictNormal);
             if (++stage == kLStages) { stage = 0; phase ^= 1; }
           }
         }
         wait_seq_ge(cready, static_cast<uint32_t>(k + 1), ab);  // the watcher (warp 2) has seen counter (t-1, g)
-        if (t > 0) fence_proxy_async();  // h_{t-1} was written through the generic proxy, TMA reads it
+        if (t > a.t_begin) fence_proxy_async();  // h_{t-1} was written through the generic proxy, TMA reads it
         IE_TRACE(0, k);
         for (int kb = 0; kb < nkt; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1, ab);
-          if (crank == 0) mbar_arrive_expect_tx(&full[stage], 2 * a_bytes);
-          else mbar_arrive_remote(&full[stage], leader);
+          mbar_arrive_expect_tx(&full[stage], kHBytes);
           const int seg = kb / a.nkb, r = kb - seg * a.nkb;            // split-bf16: [h_hi | h_lo | h_hi]
+          const int kc = (seg == 1 ? a.kh_pad : 0) + r * 64;
           if constexpr (MC) {
-            // quarter tile: rows [64 * cpair, +64) of this CTA's 128 rows, to this CTA and its counterpart in the sibling pair
-            tma_load_2d_pair_mc(ring + stage * stage_bytes + cpair * (a_bytes / 2), &tm_h64, &full[stage],
-                                (seg == 1 ? a.kh_pad : 0) + r * 64, row0 + static_cast<int>(cpair) * 64,
-                                static_cast<uint16_t>(0x5u << crank), kEvictNormal);
+            // this CTA's half of the rows, to the same offset in both CTAs of the cluster
+            tma_load_2d_mc(ring + stage * kStageBytes + crank * (kHBytes / 2), &tm_h64, &full[stage], kc,
+                           row0 + static_cast<int>(crank) * (kLRows / 2), static_cast<uint16_t>(0x3), kEvictNormal);
           } else {
-            tma_load_2d_pair(ring + stage * stage_bytes, &tm_h, &full[stage], (seg == 1 ? a.kh_pad : 0) + r * 64, row0,
-                             kEvictNormal);
+            tma_load_2d(ring + stage * kStageBytes, &tm_h, &full[stage], kc, row0, kEvictNormal);
           }
           if (++stage == kLStages) { stage = 0; phase ^= 1; }
         }
         IE_TRACE(1, k);
       }
-    }
-  } else if (warp == 2) {
-    // ---------------- counter watcher: runs ahead of the h producer and the epilogue ----------------------------
-    // The counter load and the gpu-scope fence after it cost ~1-2 us next to the TMA streams; done here they are off
-    // the h producer's path.
-    if (lane == 0) {
-      int k = 0;
-      for (long long n = pair; n < total && !aborted(ab); n += P, ++k) {
-        const int t = static_cast<int>(n / C);
-        const int g = static_cast<int>(n - static_cast<long long>(t) * C) / tiles;
-        if (t > 0) wait_flag_ge_relaxed(a.step_done + (t - 1) * ng + g, batch_ctas, ab);  // ends with a gpu-scope fence
-        st_release_cta(cready, static_cast<uint32_t>(k + 1));
-      }
-    }
-  } else if (warp == 3) {
-    // ---------------- W producer: free-running ahead of h ----------------------------------------------------
-    if (lane == 0) {
+    } else if (warp == 1 && lane == 0) {
+      // ---------------- W producer: free-running ahead of h ----------------------------------------------------
       int stage = 0;
       uint32_t phase = 0;
-      for (long long n = pair; n < total && !aborted(ab); n += P) {
-        const int j = static_cast<int>(n % C) % tiles;
-        const int wrow0 = (2 * j + static_cast<int>(crank)) * kLHalfRows;  // slices are [cta][unit][gate], 128 rows each
+      for (long long n = blockIdx.x; n < total && !aborted(ab); n += P) {
+        int t, g, half, j;
+        decode(n, t, g, half, j);
         for (int kb = 0; kb < pre + nkt; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1, ab);
-          if (crank == 0) mbar_arrive_expect_tx(&full[stage], 2 * w_bytes);
-          else mbar_arrive_remote(&full[stage], leader);
+          mbar_arrive_expect_tx(&full[stage], kWBytes);
           const int seg = FUSE ? 0 : kb / a.nkb, r = kb - seg * a.nkb;  // split-bf16: [W_hi | W_hi | W_lo]; FUSE: [W_ih | W_hh]
-          tma_load_2d_pair(ring + stage * stage_bytes + a_bytes, &tm_w, &full[stage], (seg == 2 ? a.kh_pad : 0) + r * 64,
-                           wrow0, kEvictLast);
+          tma_load_2d(ring + stage * kStageBytes + kHBytes, &tm_w, &full[stage], (seg == 2 ? a.kh_pad : 0) + r * 64,
+                      j * kLTileN, kEvictLast);
           if (++stage == kLStages) { stage = 0; phase ^= 1; }
         }
       }
-    }
-  } else if (warp == 1) {
-    // ---------------- UMMA issuer (leader CTA) --------------------------------------------------------------
-    if (crank == 0 && lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(256, kLTileN);
-      const uint32_t ring_base = smem_u32(ring);
-      int st = 0;
-      uint32_t ph = 0;
+    } else if (warp == 2 && lane == 0) {
+      // ---------------- counter watcher: runs ahead of the h producer and the epilogue ----------------------------
       int k = 0;
-      for (long long n = pair; n < total && !aborted(ab); n += P, ++k) {
-        const int slot = k & 1;
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(slot * kLTileN);
-        long long wa = 0, t_first = 0;
-        if (k >= 2) {  // the slot's previous item (k - 2) must have been read out of TMEM by both CTAs
-          const long long c0 = trace ? clock64() : 0;
-          mbar_wait(&tempty[slot], static_cast<uint32_t>(((k >> 1) - 1) & 1), ab);
-          IE_TRACE_VAL(11, k, trace ? clock64() - c0 : 0);
-        }
-        for (int kb = 0; kb < pre + nkt; ++kb) {
-          const long long c0 = trace ? clock64() : 0;
-          mbar_wait(&full[st], ph, ab);
-          if (kb == 0) t_first = trace ? clock64() : 0;
-          if (kb == pre) IE_TRACE(2, k);                               // first h_{t-1} stage landed
-          else if (trace) wa += clock64() - c0;
-          tc_fence_after();
-          const uint64_t da = umma_desc_sw128(ring_base + st * stage_bytes);
-          const uint64_t db = umma_desc_sw128(ring_base + st * stage_bytes + a_bytes);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) umma_bf16_pair(tmem_d, da + 2 * q, db + 2 * q, idesc, (kb | q) != 0);
-          umma_commit_pair_mc(&empty[st], emask);
-          if (++st == kLStages) { st = 0; ph ^= 1; }
-        }
-        umma_commit_pair_mc(&tfull[slot], pmask);
-        IE_TRACE(3, k);
-        IE_TRACE_VAL(8, k, wa);                                        // SM cycles waiting for operand stages
-        IE_TRACE_VAL(9, k, 0);
-        IE_TRACE_VAL(10, k, trace ? clock64() - t_first : 0);
+      for (long long n = blockIdx.x; n < total && !aborted(ab); n += P, ++k) {
+        int t, g, half, j;
+        decode(n, t, g, half, j);
+        if (t > a.t_begin)   // ends with a gpu-scope fence
+          wait_flag_ge_relaxed(a.step_done + (t - a.t_begin - 1) * ng + g, static_cast<unsigned>(per_batch), ab);
+        st_release_cta(cready, static_cast<uint32_t>(k + 1));
       }
     }
-  } else if (warp >= 4) {
-    // ---------------- epilogue (never leaves its loop early: named barriers inside; in drain mode its waits return
-    //                  at once and it runs through the remaining items) -----------------------------------------------
-    const int e = warp - 4;
-    const int q = e & 3;
-    const int cq = e >> 2;  // which 64 of the tile's 256 columns (4 chunks of 16 = 16 hidden units per thread)
-    const int row = static_cast<int>(crank) * 128 + q * 32 + lane;
+  } else {
+    // ---------------- consumers: MMA + epilogue (never leave their loop early: named barriers inside; in drain mode
+    //                  their waits return at once and they run through the remaining items) ------------------------
+    const int wg = (warp - 4) >> 2;              // which 64 rows of the item
+    const int q = lane & 3;
+    const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     const long long lo_off = a.segs > 1 ? a.kh_pad : 0;
+    const uint32_t ring_base = smem_u32(ring);
+    const bool signal = (threadIdx.x & 127) == 0;
+    int stage = 0;
+    uint32_t phase = 0;
     int k = 0;
-    for (long long n = pair; n < total; n += P, ++k) {
-      const int t = static_cast<int>(n / C);
-      const int c = static_cast<int>(n - static_cast<long long>(t) * C);
-      const int g = c / tiles, j = c % tiles;
+    float d[128];
+    for (long long n = blockIdx.x; n < total; n += P, ++k) {
+      int t, g, half, j;
+      decode(n, t, g, half, j);
       const int tg = a.t0 + t;  // global timestep
-      const int slot = k & 1;
-      const int brow = g * 256 + row;
-      const int unit0 = j * 64 + cq * 16;
-      const int len = POOL ? a.lengths[brow] : 1;
-      const long long grow = TOK ? static_cast<long long>(__ldg(a.tok + static_cast<long long>(tg) * b_pad + brow))
-                                 : static_cast<long long>(t) * b_pad + brow;  // TOK: per-token projection table
-      float* cp = a.cstate + static_cast<long long>(brow) * a.out_pad + unit0;
-      __nv_bfloat16* yrow = a.y + (static_cast<long long>(t + 1) * b_pad + brow) * a.ldy + unit0;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(slot * kLTileN + cq * 64);
-      // all of this thread's Gx (4 chunks x 4 units x 4 gates) and c are loaded while the MMAs still run
-      constexpr int kCh = 4;
-      constexpr int kGW = GXBF ? 8 : 16;   // 32-bit words of Gx per chunk
-      [[maybe_unused]] uint32_t gxw[FUSE ? 1 : kCh][FUSE ? 1 : kGW];
-      float4 cr[kCh];
-      [[maybe_unused]] const float4* bias4 = FUSE ? reinterpret_cast<const float4*>(a.bias + 4ll * unit0) : nullptr;
-      if constexpr (FUSE) {
-        // nothing to stream: the bias (the same 64 floats for every row of the warp) is read chunk by chunk below
-      } else if constexpr (GXBF) {
-        const __half* gxp = reinterpret_cast<const __half*>(a.gx) + grow * (4ll * a.out_pad) + 4ll * unit0;
+      int prev = -1;
+      for (int kb = 0; kb < pre + nkt; ++kb) {
+        mbar_wait(&full[stage], phase, ab);
+        if (kb == pre && signal && wg == 0) IE_TRACE(2, k);          // first h_{t-1} stage landed
+        const uint32_t sa = ring_base + stage * kStageBytes;
+        const uint64_t da = wgmma_desc_sw128(sa + wg * (kHBytes / 2));
+        const uint64_t db = wgmma_desc_sw128(sa + kHBytes);
+        wgmma_fence();
 #pragma unroll
-        for (int ch = 0; ch < kCh; ++ch) ldg_stream8_b32(gxp + ch * 16, &gxw[ch][0]);
-      } else {
-        const float* gxp = reinterpret_cast<const float*>(a.gx) + grow * (4ll * a.out_pad) + 4ll * unit0;
-#pragma unroll
-        for (int ch = 0; ch < kCh; ++ch) {
-          ldg_stream8_b32(gxp + ch * 16, &gxw[ch][0]);
-          ldg_stream8_b32(gxp + ch * 16 + 8, &gxw[ch][kGW - 8]);
+        for (int kk = 0; kk < 4; ++kk) wgmma_m64n256k16(d, da + 2 * kk, db + 2 * kk, (kb | kk) != 0);
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          if (signal) {
+            mbar_arrive(&empty[prev]);
+            if (MC) mbar_arrive_remote(&empty[prev], crank ^ 1u);
+          }
         }
+        prev = stage;
+        if (++stage == kLStages) { stage = 0; phase ^= 1; }
       }
-      // c_{t-1} of this chain was written by another pair: read it (from L2) only after (t-1, g) has been seen here
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      if (signal && prev >= 0) {
+        mbar_arrive(&empty[prev]);
+        if (MC) mbar_arrive_remote(&empty[prev], crank ^ 1u);
+      }
+      if (signal && wg == 0) IE_TRACE(3, k);
+      // c_{t-1} of this chain was written by another CTA: read it (from L2) only after (t-1, g) has been seen here
       if (lane == 0) wait_seq_ge(cready, static_cast<uint32_t>(k + 1), ab);
       __syncwarp();
 #pragma unroll
-      for (int ch = 0; ch < kCh; ch += 2) {   // full-sector (256-bit) loads
-        if (tg == 0) cr[ch] = cr[ch + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
-        else ldg_cg8(cp + ch * 4, cr[ch], cr[ch + 1]);
-      }
-      // last layer: the running max travels like c (L2, loaded before the accumulator is ready); the sum is an L2 reduction
-      [[maybe_unused]] float4 pm[POOL ? kCh : 1];
-      [[maybe_unused]] const long long po = static_cast<long long>(brow) * a.out_pad + unit0;
-      if constexpr (POOL) {
-        if (tg > 0 && tg < len) {
+      for (int hr = 0; hr < 2; ++hr) {
+        const int brow = g * 256 + half * kLRows + rbase + 8 * hr;
+        const int len = POOL ? a.lengths[brow] : 1;
+        const long long grow = TOK ? static_cast<long long>(__ldg(a.tok + static_cast<long long>(tg) * b_pad + brow))
+                                   : static_cast<long long>(t) * b_pad + brow;  // TOK: per-token projection table
+        const int unit0 = j * 64 + q;
+        float* cp = a.cstate + static_cast<long long>(brow) * a.out_pad + unit0;
+        __nv_bfloat16* yrow = a.y + (static_cast<long long>(t + 1) * b_pad + brow) * a.ldy + unit0;
+        const long long po = static_cast<long long>(brow) * a.out_pad + unit0;
+        const long long gbase = grow * (4ll * a.out_pad) + j * kLTileN + 2 * q;
 #pragma unroll
-          for (int ch = 0; ch < kCh; ch += 2) ldg_cg8(a.pool_max + po + ch * 4, pm[ch], pm[ch + 1]);
-        }
-      }
-      if (threadIdx.x == 128) IE_TRACE(7, k);
-      mbar_wait(&tfull[slot], static_cast<uint32_t>((k >> 1) & 1), ab);
-      tc_fence_after();
-      if (threadIdx.x == 128) IE_TRACE(4, k);
-      // Results of two chunks (8 units) leave with full-sector 256-bit stores: a thread owns one row, so every store
-      // instruction of a warp touches 32 different rows -- 16-byte c / 8-byte h pieces cost four L2 write transactions
-      // per sector instead of one, and the ~8000 store transactions per item were what the epilogue spent its time on.
-      uint32_t hp[8];        // bf16 h of the thread's 16 units, packed
-      float cbuf[8];         // c of the current chunk pair
-      [[maybe_unused]] float mbuf[8];
-#pragma unroll
-      for (int ch = 0; ch < kCh; ++ch) {
-        uint32_t r[16];
-        __syncwarp();
-        tmem_ld16(taddr + ch * 16, r);
-        tmem_ld_wait();
-        float4 gx4[4];
-        if constexpr (FUSE) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) gx4[u] = __ldg(bias4 + ch * 4 + u);
-        } else if constexpr (GXBF) {
-          gx_unpack_f16(gxw[ch], gx4);
-        } else {
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            gx4[u] = make_float4(__uint_as_float(gxw[ch][4 * u]), __uint_as_float(gxw[ch][4 * u + 1]),
-                                 __uint_as_float(gxw[ch][4 * u + 2]), __uint_as_float(gxw[ch][4 * u + 3]));
-        }
-        const float cprev[4] = {cr[ch].x, cr[ch].y, cr[ch].z, cr[ch].w};
-        float cnew[4], hn[4];
-        lstm_cell4(r, gx4, cprev, cnew, hn, a.gate_mode);
-        const int hb = (ch & 1) * 4;
-#pragma unroll
-        for (int u = 0; u < 4; ++u) cbuf[hb + u] = cnew[u];
-        hp[2 * ch] = pack_bf16x2(hn[0], hn[1]);
-        hp[2 * ch + 1] = pack_bf16x2(hn[2], hn[3]);
-        if (lo_off > 0) {   // split-bf16 mode: the residual h - bf16(h) goes to the lo half of the ring row
-          const float2 fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&hp[2 * ch]));
-          const float2 fb = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&hp[2 * ch + 1]));
-          *reinterpret_cast<uint2*>(yrow + lo_off + ch * 4) =
-              make_uint2(pack_bf16x2(hn[0] - fa.x, hn[1] - fa.y), pack_bf16x2(hn[2] - fb.x, hn[3] - fb.y));
-        }
-        if (a.raw != nullptr) {
-          float4* rp = reinterpret_cast<float4*>(a.raw + (static_cast<long long>(brow) * a.T_total + tg) * a.raw_ld + unit0 + ch * 4);
-          *rp = make_float4(hn[0], hn[1], hn[2], hn[3]);
-        }
-        if constexpr (POOL) {
-          pool_sum_last4(a.pool_sum, a.pool_last, po + ch * 4, hn, tg, len);
-          const float mp[4] = {pm[ch].x, pm[ch].y, pm[ch].z, pm[ch].w};
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mbuf[hb + u] = (tg == 0) ? hn[u] : fmaxf(mp[u], hn[u]);
-        }
-        if (ch & 1) {
-          st_global_cg_v8(cp + (ch - 1) * 4, __float_as_uint(cbuf[0]), __float_as_uint(cbuf[1]), __float_as_uint(cbuf[2]),
-                          __float_as_uint(cbuf[3]), __float_as_uint(cbuf[4]), __float_as_uint(cbuf[5]),
-                          __float_as_uint(cbuf[6]), __float_as_uint(cbuf[7]));
-          if constexpr (POOL) {
-            if (tg < len)
-              st_global_cg_v8(a.pool_max + po + (ch - 1) * 4, __float_as_uint(mbuf[0]), __float_as_uint(mbuf[1]),
-                              __float_as_uint(mbuf[2]), __float_as_uint(mbuf[3]), __float_as_uint(mbuf[4]),
-                              __float_as_uint(mbuf[5]), __float_as_uint(mbuf[6]), __float_as_uint(mbuf[7]));
+        for (int m = 0; m < 16; ++m) {
+          // this thread's unit 4m+q of the tile: (i, f) at columns 16m + 2q (+1), (g, o) at 16m + 8 + 2q (+1)
+          float2 gif, ggo;
+          if constexpr (FUSE) {
+            gif = __ldg(reinterpret_cast<const float2*>(a.bias + j * kLTileN + 2 * q + 16 * m));
+            ggo = __ldg(reinterpret_cast<const float2*>(a.bias + j * kLTileN + 2 * q + 16 * m + 8));
+          } else if constexpr (GXBF) {
+            const __half2* gp = reinterpret_cast<const __half2*>(reinterpret_cast<const __half*>(a.gx) + gbase + 16 * m);
+            gif = __half22float2(__ldcs(gp));
+            ggo = __half22float2(__ldcs(gp + 4));
+          } else {
+            const float2* gp = reinterpret_cast<const float2*>(reinterpret_cast<const float*>(a.gx) + gbase + 16 * m);
+            gif = __ldcs(gp);
+            ggo = __ldcs(gp + 4);
           }
+          const float zi = d[8 * m + 2 * hr] + gif.x;
+          const float zf = d[8 * m + 2 * hr + 1] + gif.y;
+          const float zg = d[8 * m + 4 + 2 * hr] + ggo.x;
+          const float zo = d[8 * m + 4 + 2 * hr + 1] + ggo.y;
+          const float cprev = (tg == 0) ? 0.0f : __ldcg(cp + 4 * m);
+          float cnew, hn;
+          lstm_cell1(zi, zf, zg, zo, cprev, cnew, hn, a.gate_mode);
+          __stcg(cp + 4 * m, cnew);
+          store_h1(yrow + 4 * m, hn, lo_off);
+          if (a.raw != nullptr)
+            a.raw[(static_cast<long long>(brow) * a.T_total + tg) * a.raw_ld + unit0 + 4 * m] = hn;
+          if constexpr (POOL) pool_accumulate1(a.pool_sum, a.pool_max, a.pool_last, po + 4 * m, hn, tg, len);
         }
       }
-      st_global_v8(yrow, hp[0], hp[1], hp[2], hp[3], hp[4], hp[5], hp[6], hp[7]);   // h_t: 16 units = one 32-byte sector
-      // publish (step t, batch g): accumulator slot drained, h_t / c_t / pooling state visible
-      if (threadIdx.x == 128) IE_TRACE(5, k);
-      tc_fence_before();
-      named_bar_sync(1, 512);
+      // publish (step t, batch g): h_t / c_t / pooling state visible
+      named_bar_sync(1, 256);
       if (threadIdx.x == 128) {
-        mbar_arrive_remote(&tempty[slot], leader);
         __threadfence();
-        // fault injection for the abort-protocol test (IE_DEBUG_FAULT): item (t=1, g=0, j=0) is never published
-        if (!(a.fault && n == C)) red_relaxed_add(a.step_done + t * ng + g, 1u);
+        // fault injection for the abort-protocol test (IE_DEBUG_FAULT): item (t=1, g=0, first tile) is never published
+        if (a.step_done != nullptr && !(a.fault && n == C))
+          red_relaxed_add(a.step_done + (t - a.t_begin) * ng + g, 1u);
         IE_TRACE(6, k);
       }
     }
   }
 
   __syncwarp();
-  tc_fence_before();
-  cluster_sync();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
-  }
+  if (MC) cluster_sync();   // no CTA leaves while its sibling may still multicast into it or arrive on its barriers
   if (a.diag != nullptr && threadIdx.x == 0 && blockIdx.x == 0) {
     unsigned long long g;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
@@ -456,13 +343,12 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
     a.diag[3] = static_cast<long long>(g);
   }
 #undef IE_TRACE
-#undef IE_TRACE_VAL
 }
 
-thread_local int g_last_max_pairs = 0;   // result of the last check_only query on this thread
+thread_local int g_last_max_ctas = 0;   // result of the last check_only query on this thread
 
 template <bool TOK, bool GXBF, bool POOL>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kLThreads, 1)
+__global__ void __launch_bounds__(kLThreads, 1)
 lstm_layer_kernel(const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_w,
                   const __grid_constant__ CUtensorMap tm_h64, const __grid_constant__ CUtensorMap tm_x,
                   const __grid_constant__ KArgs a) {
@@ -471,7 +357,7 @@ lstm_layer_kernel(const __grid_constant__ CUtensorMap tm_h, const __grid_constan
 
 // input projection fused into the K loop (the last layer by default; see FUSE above)
 template <bool POOL>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kLThreads, 1)
+__global__ void __launch_bounds__(kLThreads, 1)
 lstm_layer_fused_kernel(const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_w,
                         const __grid_constant__ CUtensorMap tm_h64, const __grid_constant__ CUtensorMap tm_x,
                         const __grid_constant__ KArgs a) {
@@ -479,19 +365,17 @@ lstm_layer_fused_kernel(const __grid_constant__ CUtensorMap tm_h, const __grid_c
 }
 
 template <bool TOK>
-__global__ void __launch_bounds__(kLThreads, 1)
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kLThreads, 1)
 lstm_layer_mc_kernel(const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_w,
                      const __grid_constant__ CUtensorMap tm_h64, const __grid_constant__ CUtensorMap tm_x,
                      const __grid_constant__ KArgs a) {
   lstm_layer_body<TOK, true, false, true, false>(tm_h, tm_w, tm_h64, tm_x, a);
 }
 
-size_t layer_smem_bytes() {
-  return 1024 + static_cast<size_t>(kLStages) * (128 * 64 * 2 + kLHalfRows * 64 * 2) + (2 * kLStages + 4) * 8 + 32;
-}
+size_t layer_smem_bytes() { return 1024 + static_cast<size_t>(kLStages) * kStageBytes + 2 * kLStages * 8 + 32; }
 
 template <bool TOK, bool GXBF, bool POOL, bool MC, bool FUSE = false>
-cudaError_t launch_layer_t(const LstmLayerArgs& a, int pairs, int tiles, cudaStream_t stream) {
+cudaError_t launch_layer_t(const LstmLayerArgs& a, int ctas, int tiles, cudaStream_t stream) {
   void (*kfn)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, KArgs);
   if constexpr (MC) kfn = lstm_layer_mc_kernel<TOK>;
   else if constexpr (FUSE) kfn = lstm_layer_fused_kernel<POOL>;
@@ -500,93 +384,96 @@ cudaError_t launch_layer_t(const LstmLayerArgs& a, int pairs, int tiles, cudaStr
   // function attributes are per device: set on every launch (cheap), never cached in a process-wide flag
   cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
-  if (MC) {
-    e = cudaFuncSetAttribute(kfn, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
-    if (e != cudaSuccess) return e;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * (a.check_only ? a.num_sms / 2 : pairs));
-  cfg.blockDim = dim3(kLThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (MC) {   // the production kernel carries __cluster_dims__(2, 1, 1)
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = 4;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = na;
   if (a.check_only) {
-    // how many CTA pairs can be co-resident with this cluster shape (returned through a.check_only's contract: the
-    // caller reads lstm_layer_max_pairs())
-    if (MC) cfg.gridDim = dim3(4 * (a.num_sms / 4));
-    int max_clusters = 0;
-    e = cudaOccupancyMaxActiveClusters(&max_clusters, kfn, &cfg);
+    // how many CTAs can be co-resident (the caller reads lstm_layer_max_ctas())
+    int max_ctas = 0;
+    if (MC) {
+      cudaLaunchConfig_t cfg{};
+      cfg.gridDim = dim3(2 * (a.num_sms / 2));
+      cfg.blockDim = dim3(kLThreads);
+      cfg.dynamicSmemBytes = smem;
+      cfg.stream = stream;
+      int clusters = 0;
+      e = cudaOccupancyMaxActiveClusters(&clusters, kfn, &cfg);
+      max_ctas = 2 * clusters;
+    } else {
+      int per_sm = 0;
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kfn, kLThreads, smem);
+      max_ctas = per_sm * a.num_sms;
+    }
     if (e != cudaSuccess) return e;
-    g_last_max_pairs = max_clusters * (MC ? 2 : 1);
-    if (MC) return max_clusters >= 1 ? cudaSuccess : cudaErrorCooperativeLaunchTooLarge;
-    return max_clusters >= a.num_sms / 2 ? cudaSuccess : cudaErrorCooperativeLaunchTooLarge;
+    g_last_max_ctas = max_ctas;
+    if (MC) return max_ctas >= 2 ? cudaSuccess : cudaErrorCooperativeLaunchTooLarge;
+    return max_ctas >= a.num_sms ? cudaSuccess : cudaErrorCooperativeLaunchTooLarge;
   }
   KArgs k{};
   k.gx = a.gx; k.tok = a.tok; k.bias = a.bias; k.pre_nkb = FUSE ? a.pre_nkb : 0; k.cstate = a.c; k.y = a.y; k.raw = a.raw;
   k.pool_sum = a.pool_sum; k.pool_max = a.pool_max; k.pool_last = a.pool_last; k.lengths = a.lengths;
-  k.step_done = a.step_done; k.abort_flag = a.abort_flag;
+  k.step_done = a.single_step ? nullptr : a.step_done; k.abort_flag = a.abort_flag;
   k.spin_limit = a.spin_limit > 0 ? a.spin_limit : kSpinLimitDefault;
   k.ldy = a.ldy; k.raw_ld = a.raw_ld; k.trace = a.trace; k.diag = a.diag;
-  k.T = a.T; k.t0 = a.t0; k.T_total = a.T_total; k.ng = a.ng; k.tiles = tiles; k.out_pad = a.out_pad;
+  k.T = a.single_step ? 1 : a.T; k.t_begin = a.single_step ? a.t_step : 0;
+  k.t0 = a.t0; k.T_total = a.T_total; k.ng = a.ng; k.tiles = tiles; k.out_pad = a.out_pad;
   k.nkb = a.kh_pad / 64; k.segs = a.segs; k.kh_pad = a.kh_pad; k.gate_mode = a.gate_mode;
   k.trace_items = a.trace_items; k.fault = a.fault;
-  if (a.cooperative) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(ctas);
+  cfg.blockDim = dim3(kLThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  int na = 0;
+  if (a.cooperative && !a.single_step) {
     attr[na].id = cudaLaunchAttributeCooperative;
     attr[na].val.cooperative = 1;
     ++na;
   }
+  cfg.attrs = attr;
   cfg.numAttrs = na;
   return cudaLaunchKernelEx(&cfg, kfn, a.tm_h, a.tm_w, a.tm_h64, FUSE ? a.tm_x : a.tm_h, k);
 }
 
+// multicast needs sibling CTAs to hold items of the same (timestep, batch, row half): tiles (hence C and the item
+// total) even
+bool lstm_layer_mc_ok(const LstmLayerArgs& a) {
+  return a.mc != 0 && !a.single_step && a.gx_bf16 && a.pool_sum == nullptr && a.pre_nkb == 0 && a.segs == 1 &&
+         (a.n_cta / 2) % 2 == 0 && a.mc_ctas >= 2;
+}
+
 }  // namespace
 
-int lstm_layer_max_pairs() { return g_last_max_pairs; }
+int lstm_layer_max_ctas() { return g_last_max_ctas; }
 
-// multicast needs sibling pairs to hold items of the same (timestep, batch): tiles (hence C and the item total) even
-bool lstm_layer_mc_ok(const LstmLayerArgs& a) {
-  return a.mc != 0 && a.gx_bf16 && a.pool_sum == nullptr && a.pre_nkb == 0 && a.segs == 1 && (a.n_cta / 2) % 2 == 0 &&
-         a.mc_pairs >= 2;
+int lstm_layer_ctas(const LstmLayerArgs& a) {
+  const long long per_step = static_cast<long long>(a.ng) * a.n_cta;   // 2 row halves x n_cta / 2 tiles
+  if (a.single_step) return static_cast<int>(per_step);                // one item per CTA
+  const long long total = a.T * per_step;
+  long long ctas = lstm_layer_mc_ok(a) ? a.mc_ctas : a.num_sms;
+  if (ctas > total) ctas = total;
+  if (lstm_layer_mc_ok(a)) ctas &= ~1ll;
+  return static_cast<int>(ctas);
 }
 
-int lstm_layer_pairs(const LstmLayerArgs& a) {
-  const long long total = static_cast<long long>(a.T) * a.ng * (a.n_cta / 2);
-  long long pairs = lstm_layer_mc_ok(a) ? a.mc_pairs : a.num_sms / 2;
-  if (pairs > total) pairs = total;
-  if (lstm_layer_mc_ok(a)) pairs &= ~1ll;
-  return static_cast<int>(pairs);
-}
-
-// a.check_only: only query co-residency (lstm_layer_max_pairs()).  Requires u == 32 per CTA (64 units per pair tile).
+// a.check_only: only query co-residency (lstm_layer_max_ctas()).  Requires u == 32 per slice (64 units per tile).
 cudaError_t launch_lstm_layer(const LstmLayerArgs& a, cudaStream_t stream) {
   if (a.u != 32 || a.n_cta % 2 || a.kh_pad % 64 || a.ng < 1 || a.ng > kMaxBatches || a.T < 1 || (a.segs != 1 && a.segs != 3))
     return cudaErrorInvalidValue;
   const int tiles = a.n_cta / 2;
   if (a.check_only && a.mc) return launch_layer_t<false, true, false, true>(a, 0, tiles, stream);
-  const int pairs = lstm_layer_pairs(a);
-  if (pairs < 1) return cudaErrorInvalidValue;
+  const int ctas = lstm_layer_ctas(a);
+  if (ctas < 1) return cudaErrorInvalidValue;
   const bool tok = a.tok != nullptr;  // layer 0 reading its input projection from the per-token table
   const bool pool = a.pool_sum != nullptr;
   if (a.pre_nkb > 0) {  // input projection fused into the K loop: tm_w covers [W_ih | W_hh], tm_x the previous layer's ring
-    if (a.check_only || tok || a.segs != 1 || a.bias == nullptr) return cudaErrorInvalidValue;
-    return pool ? launch_layer_t<false, true, true, false, true>(a, pairs, tiles, stream)
-                : launch_layer_t<false, true, false, false, true>(a, pairs, tiles, stream);
+    if (a.check_only || tok || a.segs != 1 || a.bias == nullptr || a.single_step) return cudaErrorInvalidValue;
+    return pool ? launch_layer_t<false, true, true, false, true>(a, ctas, tiles, stream)
+                : launch_layer_t<false, true, false, false, true>(a, ctas, tiles, stream);
   }
   if (!a.check_only && lstm_layer_mc_ok(a))
-    return tok ? launch_layer_t<true, true, false, true>(a, pairs, tiles, stream)
-               : launch_layer_t<false, true, false, true>(a, pairs, tiles, stream);
+    return tok ? launch_layer_t<true, true, false, true>(a, ctas, tiles, stream)
+               : launch_layer_t<false, true, false, true>(a, ctas, tiles, stream);
 #define IE_LAYER(T_, G_)                                                                                  \
-  (pool ? launch_layer_t<T_, G_, true, false>(a, pairs, tiles, stream) : launch_layer_t<T_, G_, false, false>(a, pairs, tiles, stream))
+  (pool ? launch_layer_t<T_, G_, true, false>(a, ctas, tiles, stream) : launch_layer_t<T_, G_, false, false>(a, ctas, tiles, stream))
   if (a.gx_bf16) return tok ? IE_LAYER(true, true) : IE_LAYER(false, true);
   return tok ? IE_LAYER(true, false) : IE_LAYER(false, false);
 #undef IE_LAYER

@@ -219,7 +219,7 @@ cudaError_t launch_convert_rows(const float* src, long long ld_src, int cols, co
 cudaError_t launch_fill_f32(float* p, size_t n, float v, cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
   size_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   fill_f32_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(p, n, v);
   return cudaGetLastError();
 }

@@ -1,4 +1,4 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM).
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), clusters, wgmma.
 // Everything the kernels in this directory need and nothing else.  No CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
@@ -17,18 +17,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // ----------------------------------------------------------------------------------------------
 // mbarrier
 // ----------------------------------------------------------------------------------------------
@@ -38,7 +26,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// make generic-proxy writes visible to the async proxy (TMA / UMMA operand reads)
+// make generic-proxy writes visible to the async proxy (TMA operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
@@ -60,6 +48,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "r"(smem_u32(bar)), "r"(parity)
       : "memory");
   return ok != 0;
+}
+// plain arrive on the barrier at the same smem offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t"
+      ".reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
+      "}\n"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
 }
 // ----------------------------------------------------------------------------------------------
 // Abort protocol of every spin in this directory.  A wait that exceeds `limit` SM cycles (a protocol bug, or a
@@ -135,44 +134,12 @@ __device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap
       : "memory");
 }
 
-// 2-D tiled store shared -> global (bulk async group); out-of-range parts of the box are clipped by the tensor map
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-// same with an L2 cache-policy hint (evict-first: an output stream must not displace the operand panels in L2)
-__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1,
-                                                  uint64_t hint) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
-               ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "l"(hint)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// wait until at most N of this thread's bulk groups still READ their shared-memory source / are incomplete
-template <int N> __device__ __forceinline__ void bulk_wait_group_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N> __device__ __forceinline__ void bulk_wait_group() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-// make generic-proxy shared-memory writes visible to the async proxy (TMA store source)
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
 // ----------------------------------------------------------------------------------------------
 // thread-block clusters
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_nctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
   return r;
 }
 // all threads of all CTAs in the cluster (also orders shared-memory accesses like __syncthreads)
@@ -182,245 +149,78 @@ __device__ __forceinline__ void cluster_sync() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, UMMA issue, commit, TMEM loads
+// wgmma (warpgroup MMA)
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// whole warp; ncols power of two >= 32; the TMEM base address is written to *smem_dst
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// Shared-memory matrix descriptor: K-major operand tile, 128-byte swizzle, rows 128 B apart,
-// 8-row core-matrix groups 1024 B apart (what a TMA box {64 bf16, rows} with SWIZZLE_128B writes).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// Shared-memory matrix descriptor: K-major operand tile, 128-byte swizzle, rows 128 B apart, 8-row core-matrix groups
+// 1024 B apart (what a TMA box {64 bf16, rows} with SWIZZLE_128B writes).  Advancing 16 bf16 = 32 B along K inside
+// the swizzle atom is +2 in the (addr >> 4) field.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);  // [0,14)  start address >> 4
-  // [16,30) leading byte offset: unused for swizzled K-major
+  d |= 1ull << 16;                                          // [16,30) leading byte offset: unused for swizzled K-major
   d |= static_cast<uint64_t>(1024u >> 4) << 32;             // [32,46) stride byte offset >> 4
-  d |= 1ull << 46;                                          // [46,48) descriptor version (sm_100)
-  d |= 2ull << 61;                                          // [61,64) SWIZZLE_128B
+  d |= 1ull << 62;                                          // [62,64) SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16: A,B = bf16 K-major, D = f32, shape M x N (K = 16 per instruction).
-__device__ __forceinline__ uint32_t umma_idesc_bf16(uint32_t M, uint32_t N) {
-  uint32_t d = 0;
-  d |= 1u << 4;          // D format f32
-  d |= 1u << 7;          // A format bf16
-  d |= 1u << 10;         // B format bf16
-  d |= (N >> 3) << 17;   // N / 8
-  d |= (M >> 4) << 24;   // M / 16
-  return d;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]^T ; single issuing thread
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+// keep the compiler from moving accumulator reads/writes across the asynchronous MMAs
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T: both operands K-major bf16 in shared memory (descriptors above), f32
+// accumulators in the registers of the issuing warpgroup.  Fragment layout: d[4 j + {0, 1, 2, 3}] holds rows
+// {r, r, r + 8, r + 8} and columns 8 j + 2 (lane % 4) + {0, 1, 0, 1}, where r = 16 (warp % 4) + lane / 4.
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t"
       "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued UMMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// same, arriving on the barrier at the same offset in every CTA of `mask` (operand stages filled by multicast TMA
-// may only be overwritten once every CTA of the cluster has consumed them)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants: two CTAs of a cluster on one TPC act as one M=256 tensor core.
-// Barriers that gate the MMA live in the even ("leader") CTA; shared-window addresses carry the pair rank in
-// bit 24, so clearing it redirects a barrier operand to the leader's copy of the same smem offset.
-// ----------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
-// 2-D tiled load into THIS CTA's smem; the complete_tx goes to the barrier at the same offset in the leader CTA
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0,
-                                                 int32_t c1, uint64_t hint) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(m), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "l"(hint)
-      : "memory");
-}
-// multicast variant of tma_load_2d_pair: the box lands at the same CTA-relative offset in every CTA of `mask`; with
-// cta_group::2 the complete_tx of each destination goes to the barrier (same offset) of the CTA of ITS pair whose rank has
-// the parity of the CTA `bar` points to -- `bar` is redirected to this pair's leader, so every destination pair's
-// leader is signalled
-__device__ __forceinline__ void tma_load_2d_pair_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0,
-                                                    int32_t c1, uint16_t mask, uint64_t hint) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      ".L2::cache_hint [%0], [%1, {%4, %5}], [%2], %3, %6;"
-      ::"r"(smem_u32(smem_dst)), "l"(m), "r"(smem_u32(bar) & kPeerBitMask), "h"(mask), "r"(c0), "r"(c1), "l"(hint)
-      : "memory");
-}
-// plain arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-      "}\n"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A * B^T with M = 256: rows 0..127 of A and columns 0..N/2-1 of B come from the leader's
-// smem, the other halves from the peer's smem at the same offsets.  Issued by one thread of the leader CTA.
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit of the pair's MMAs, arriving on the barrier at the same offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_pair_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(mask)
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------
 // grid-scope flags in global memory (persistent kernels)
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void red_release_add(unsigned* p, unsigned v) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-// bounded spin until *p >= target (abort protocol above instead of hanging the GPU on a protocol bug)
-__device__ __forceinline__ void wait_flag_ge(const unsigned* p, unsigned target, const Abort& ab) {
-  if (ld_acquire(p) >= target) return;
-  if (aborted(ab)) return;
-  const long long t0 = clock64();
-  uint32_t spins = 0;
-  while (ld_acquire(p) < target) {
-    if (((++spins) & 0x3Fu) == 0 && abort_poll(ab, t0)) return;
-  }
-}
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-// TMEM -> registers: the warp's 32 lanes x 16 consecutive 32-bit columns (thread i <- lane base+i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------------------------
-// misc
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ float sigmoid_acc(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-// tanh(x) = 1 - 2/(exp(2x)+1): abs error ~1e-7, saturates correctly for |x| large
-__device__ __forceinline__ float tanh_acc(float x) { return 1.0f - __fdividef(2.0f, __expf(2.0f * x) + 1.0f); }
-
-// single-MUFU variants (tanh.approx.f32, max relative error 2^-11): the epilogue of the recurrent kernels is bound by
-// the 16/clk/SM special-function unit (10 MUFU per cell with the accurate forms, 5 with these)
-__device__ __forceinline__ float tanh_fast(float x) {
-  float y;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
-
-// 256-bit global store (sm_100): one full 32-byte sector per instruction, so the L2 never sees a partial-sector
-// write (the 128-bit stores of the first GEMM epilogue caused read-modify-write fills: DRAM reads ~ output bytes)
-__device__ __forceinline__ void st_global_v8(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e,
-                                             uint32_t f, uint32_t g, uint32_t h) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d),
-               "r"(e), "r"(f), "r"(g), "r"(h)
-               : "memory");
-}
-
-// 256-bit store that stays out of L1 (state another SM will read from L2 with ld.global.cg)
-__device__ __forceinline__ void st_global_cg_v8(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e,
-                                                uint32_t f, uint32_t g, uint32_t h) {
-  asm volatile("st.global.cg.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d),
-               "r"(e), "r"(f), "r"(g), "r"(h)
-               : "memory");
-}
-
-// streaming 256-bit read-only load (sm_100): no L1 allocation, evict-first in L2 -- a once-read stream must not
-// displace the L2-resident weights.  (The .L2::evict_first qualifier only exists for the 256-bit forms.)
-__device__ __forceinline__ void ldg_stream8(const float* p, float4& a, float4& b) {
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w)
-               : "l"(p));
-}
-
-// 256-bit coherent load that bypasses L1 (state written by another SM of the same launch: c, running max).  One full
-// 32-byte sector per request -- two 128-bit ld.cg of the same sector are two requests and move the sector twice
-// (ncu: 6.4 GB of the recurrent kernel's 25.7 GB of LSU reads per launch were the second halves of c sectors).
-__device__ __forceinline__ void ldg_cg8(const float* p, float4& a, float4& b) {
-  asm volatile("ld.global.cg.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w)
-               : "l"(p)
-               : "memory");
-}
-
-// same load into eight 32-bit registers (f32 bits or packed bf16 pairs)
-__device__ __forceinline__ void ldg_stream8_b32(const void* p, uint32_t* d) {
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]), "=r"(d[4]), "=r"(d[5]), "=r"(d[6]), "=r"(d[7])
-               : "l"(p));
-}
-
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ unsigned ld_relaxed(const unsigned* p) {
   unsigned v;
   asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-// bounded spin with relaxed loads, one acquire fence at the end
+// bounded spin with relaxed loads, one acquire fence at the end (abort protocol above instead of hanging the GPU)
 __device__ __forceinline__ void wait_flag_ge_relaxed(const unsigned* p, unsigned target, const Abort& ab) {
   if (ld_relaxed(p) < target && !aborted(ab)) {
     const long long t0 = clock64();
@@ -434,5 +234,28 @@ __device__ __forceinline__ void wait_flag_ge_relaxed(const unsigned* p, unsigned
 __device__ __forceinline__ void red_relaxed_add(unsigned* p, unsigned v) {
   asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// misc
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+__device__ __forceinline__ float sigmoid_acc(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
+// tanh(x) = 1 - 2/(exp(2x)+1): abs error ~1e-7, saturates correctly for |x| large
+__device__ __forceinline__ float tanh_acc(float x) { return 1.0f - __fdividef(2.0f, __expf(2.0f * x) + 1.0f); }
+
+// single-MUFU variants (tanh.approx.f32, max relative error 2^-11): the epilogue of the recurrent kernel is bound by
+// the 16/clk/SM special-function unit (10 MUFU per cell with the accurate forms, 5 with these)
+__device__ __forceinline__ float tanh_fast(float x) {
+  float y;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
 
 }  // namespace ie

@@ -2,7 +2,7 @@
 
 Token ids -> 2400-d [mean | max | last] vectors, i.e. the arithmetic behind
 ``InferenceWrapper._forward_pass`` + ``batch_seq_pool`` (Issue_Embeddings/flask_app/inference.py:55-57,
-215-246) executed by the sm_100a kernels in csrc/.  torch is used only for pinned host buffers, device tensors
+215-246) executed by the sm_90a kernels in csrc/.  torch is used only for pinned host buffers, device tensors
 and streams.
 """
 from __future__ import annotations
@@ -126,8 +126,14 @@ class IssueEncoder:
         assert ids.is_cuda and lengths.is_cuda and ids.dtype == torch.int64 and lengths.dtype == torch.int32
         ids, lengths = ids.contiguous(), lengths.contiguous()
         B, T = ids.shape
+        if tuple(lengths.shape) != (B,):
+            raise ValueError(f"lengths has shape {tuple(lengths.shape)}, expected ({B},)")
         if out is None:
             out = torch.empty((B, self.out_dim), dtype=torch.float32, device=ids.device)
+        # the library writes B rows through a raw pointer: the buffer must be exactly that
+        if (not out.is_cuda or out.dtype != torch.float32 or tuple(out.shape) != (B, self.out_dim)
+                or not out.is_contiguous()):
+            raise ValueError(f"out must be a contiguous cuda float32 tensor of shape ({B}, {self.out_dim})")
         s = stream if stream is not None else torch.cuda.current_stream(ids.device)
         check(self._lib.ie_encoder_encode(self._h, ids.data_ptr(), lengths.data_ptr(), B, T, out.data_ptr(),
                                           IE_FLAG_DEVICE_PTRS, C.c_void_p(s.cuda_stream)))

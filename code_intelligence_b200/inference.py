@@ -1,5 +1,5 @@
 """Drop-in mirror of the reference's ``InferenceWrapper`` (Issue_Embeddings/flask_app/inference.py:27-246 and
-py/code_intelligence/inference.py:25-263) with the encoder arithmetic on the B200.
+py/code_intelligence/inference.py:25-263) with the encoder arithmetic on the H100.
 
 Same names, argument meaning and error behaviour:
 
@@ -11,7 +11,7 @@ Same names, argument meaning and error behaviour:
     .batch_seq_pool(seq_emb, lengths)
     pass_through                 (module level, needed to unpickle fastai learners: app.py:10)
 
-The contract of the B200 path starts at token ids (SURVEY.md section 8b), so every text-taking method has an
+The contract of the GPU path starts at token ids (SURVEY.md section 8b), so every text-taking method has an
 id-taking twin (``*_from_ids``).  Text -> ids needs the model's tokenizer + vocab: when fastai is importable the
 exported learner's own ``one_item`` / ``TextLMDataBunch`` machinery is used exactly as in the reference; otherwise
 a ``numericalizer`` callable (str -> 1-D int64 array, starting with xxbos) must be supplied, or the built-in
@@ -278,7 +278,7 @@ class InferenceWrapper:
     @classmethod
     def batch_seq_pool(cls, seq_emb, lengths):
         """Concatenate the mean, max and last hidden representations of a batch of sequences (host utility kept
-        for interface parity, inference.py:215-246; the B200 path pools on the device instead)."""
+        for interface parity, inference.py:215-246; the GPU path pools on the device instead)."""
         assert seq_emb.shape[0] == len(lengths), \
             'Number of elements in lengths should match the first dimension of seq_emb'
         seq_emb = np.asarray(seq_emb)

@@ -1,9 +1,9 @@
-"""Label_Microservice MLP head on the B200.
+"""Label_Microservice MLP head on the H100.
 
 ``MLPWrapper`` keeps the reference's interface (py/label_microservice/mlp.py:14-138) -- the constructor, ``fit``,
 ``predict_probabilities``, ``find_probability_thresholds``, ``grid_search``, ``save_model`` / ``load_model`` -- but
 ``predict_probabilities`` (mlp.py:56-63, sklearn ``MLPClassifier.predict_proba``) runs the fitted network's forward
-pass relu(relu(X W0 + b0) W1 + b1) ... -> sigmoid through the tcgen05 GEMM kernel behind ``ie_mlp_*``
+pass relu(relu(X W0 + b0) W1 + b1) ... -> sigmoid through the wgmma GEMM kernel behind ``ie_mlp_*``
 (include/issue_emb_b200.h).  Training-time methods stay on sklearn (out of scope, SURVEY.md section 2 row 5).
 """
 from __future__ import annotations
@@ -140,12 +140,12 @@ class MLPWrapper:
         self.total_labels_count = None
 
     def fit(self, X, y):
-        """Train the classifier (sklearn on the CPU: training is out of scope of the B200 path)."""
+        """Train the classifier (sklearn on the CPU: training is out of scope of the GPU path)."""
         self.clf.fit(X, y)
         self._head = None
 
     def predict_probabilities(self, X):
-        """Predict probabilities of all labels for data -> (n_samples, n_classes); on the B200."""
+        """Predict probabilities of all labels for data -> (n_samples, n_classes); on the H100."""
         if self._head is None:
             self._head = MLPHead.from_sklearn(self.clf, self._device)
         return self._head.predict_proba(X)

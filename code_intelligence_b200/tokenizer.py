@@ -2,7 +2,7 @@
 behind fastai 1.0.53's ``Tokenizer(SpacyTokenizer('en'))`` that the reference's learner uses to numericalise issues
 (Issue_Embeddings/flask_app/inference.py:51-53, :174-182; SURVEY.md section 8, row f-1 "next").
 
-Boundary code, host only; the B200 path starts at token ids.  PARITY UNPINNED: spaCy is not installed in this image, so
+Boundary code, host only; the GPU path starts at token ids.  PARITY UNPINNED: spaCy is not installed in this image, so
 the rules below are restated from the published spaCy 2.1 sources (``spacy/tokenizer.pyx`` -- the whitespace /
 prefix / suffix / infix / special-case loop; ``spacy/lang/punctuation.py`` and ``char_classes.py`` -- the character
 classes; ``spacy/lang/en/tokenizer_exceptions.py`` and ``lang/tokenizer_exceptions.py`` -- contractions,

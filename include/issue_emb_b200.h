@@ -1,4 +1,4 @@
-/* issue_emb_b200 -- C ABI of the B200-native Issue_Embeddings encoder hot path and the Label_Microservice
+/* issue_emb_b200 -- C ABI of the H100-native Issue_Embeddings encoder hot path and the Label_Microservice
  * MLP head (libissue_emb_b200.so).  Plain pointers and sizes only; no torch / C++ types.
  *
  * The reference (kubeflow/Code-Intelligence) has no FFI layer for this path: its "operator API" is the Python
@@ -154,7 +154,7 @@ int ie_pr_thresholds(const float* scores, const uint8_t* truth, int32_t n, int32
                      double recall_threshold, float* thresholds, double* precisions, double* recalls, int32_t device,
                      int32_t flags, void* stream);
 
-/* Debug / test hook: D[M,N] = A[M,K] * B[N,K]^T (+bias) through the same tcgen05 GEMM the encoder uses.
+/* Debug / test hook: D[M,N] = A[M,K] * B[N,K]^T (+bias) through the same wgmma GEMM the encoder uses.
  * a [M,K], b [N,K], bias [N] or NULL: host f32 (rounded to bf16 on the device); d [M,N] host f32. */
 int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
                   float* d, int32_t device);

@@ -63,6 +63,34 @@ def mlp_forward(X, coefs, intercepts, dtype=np.float64):
     return 1.0 / (1.0 + np.exp(-a))
 
 
+def seeded_mlp(seed, dims, n_rows):
+    """Seeded MLP head parameters (Glorot-uniform, as sklearn initialises them) and N(0, 0.1^2) inputs: the
+    production-shape fixture (tests/golden/mlp_ref_prod.npz) stores only these arguments and the reference's outputs.
+    numpy's PCG64 stream is the same on every machine."""
+    rng = np.random.default_rng(seed)
+    coefs, intercepts = [], []
+    for fan_in, fan_out in zip(dims[:-1], dims[1:]):
+        bound = np.sqrt(6.0 / (fan_in + fan_out))
+        coefs.append(rng.uniform(-bound, bound, (fan_in, fan_out)).astype(np.float32))
+        intercepts.append(rng.uniform(-bound, bound, fan_out).astype(np.float32))
+    # output biases of a head trained on labels with ~20 % base rates (what sklearn's fit gives in a few steps)
+    intercepts[-1] = rng.uniform(-1.75, -1.15, dims[-1]).astype(np.float32)
+    X = (rng.standard_normal((n_rows, dims[0])) * 0.1).astype(np.float32)
+    return coefs, intercepts, X
+
+
+def load_mlp_fixture(path):
+    """(coefs, intercepts, X, reference probabilities) of a tests/golden/mlp_ref_*.npz fixture: stored arrays, or the
+    arguments of seeded_mlp."""
+    z = np.load(path)
+    if "seed" in z.files:
+        coefs, intercepts, X = seeded_mlp(int(z["seed"]), [int(v) for v in z["dims"]], int(z["n_rows"]))
+    else:
+        n = int(z["n_layers"])
+        coefs, intercepts, X = [z[f"coef{i}"] for i in range(n)], [z[f"intercept{i}"] for i in range(n)], z["X"]
+    return coefs, intercepts, X, z["probs"]
+
+
 def filter_labels(label_names, probs, thresholds):
     """py/label_microservice/repo_specific_model.py:126-146 -- keep label iff its threshold is truthy
     and prob >= threshold."""

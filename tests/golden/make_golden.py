@@ -6,9 +6,10 @@
                      the reference's own encoder is not importable here, SURVEY.md section 8c) on seeded inputs.
                      Small configs carry their weights; the reference-shape (R4 / N3) fixtures carry only ids and
                      expected outputs -- their weights are re-derived from the seed (torch CPU RNG is deterministic).
-* mlp_ref.npz     -- produced by IMPORTING THE REFERENCE: label_microservice.mlp.MLPWrapper from /root/reference/py
-                     (py/label_microservice/mlp.py:56-63) around a fitted sklearn MLPClassifier; stores coefs_,
-                     intercepts_, inputs and MLPWrapper.predict_probabilities outputs.
+* mlp_ref_*.npz   -- produced by IMPORTING THE REFERENCE: label_microservice.mlp.MLPWrapper (py/label_microservice/mlp.py:56-63)
+                     around an sklearn MLPClassifier; 'small' stores the fitted coefs_, intercepts_, inputs and the
+                     MLPWrapper.predict_probabilities outputs, 'prod' the seed of its weights and inputs
+                     (oracle.lstm_numpy.seeded_mlp) and the outputs.
 * thresholds_ref.npz (`make_golden.py thresholds`) -- the reference's MLPWrapper.find_probability_thresholds (mlp.py:65-98)
                      executed on preset scores.
 * reference_driver.npz (`make_golden.py driver`) -- the reference's OWN bulk driver, pooling and single-issue code
@@ -24,6 +25,16 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
+# a checkout of kubeflow/code-intelligence (the reference whose own code produces the mlp / thresholds / driver fixtures)
+REFERENCE = os.environ.get('CODE_INTELLIGENCE_REFERENCE', '')
+
+
+def reference_root():
+    """The reference checkout, or a clear error: only the reference-pinned fixtures need it."""
+    if not REFERENCE or not os.path.isdir(os.path.join(REFERENCE, 'py')):
+        raise SystemExit('CODE_INTELLIGENCE_REFERENCE must name a checkout of kubeflow/code-intelligence (a directory with '
+                         'py/ and Issue_Embeddings/) to regenerate the mlp / thresholds / driver fixtures; got %r' % REFERENCE)
+    return REFERENCE
 sys.path.insert(0, ROOT)
 
 from oracle import awd_lstm_ref as R  # noqa: E402
@@ -55,29 +66,47 @@ def encoder_fixture(name, n_layers, emb_sz, n_hid, vocab, B, T, min_len, seed, s
 
 
 def mlp_fixture():
-    sys.path.insert(0, '/root/reference/py')
+    sys.path.insert(0, os.path.join(reference_root(), 'py'))
     from label_microservice.mlp import MLPWrapper  # the reference's own wrapper
     from sklearn.neural_network import MLPClassifier
+    from oracle.lstm_numpy import seeded_mlp
+    import warnings
     rng = np.random.default_rng(1234)
-    for tag, d_in, hidden, n_labels, n_train, n_test in [('small', 24, (32, 16), 5, 200, 64),
-                                                         ('prod', 1600, (600, 600), 40, 256, 96)]:
-        X = (rng.standard_normal((n_train, d_in)) * 0.1).astype(np.float32)
-        Y = (rng.random((n_train, n_labels)) < 0.2).astype(int)
-        Xt = (rng.standard_normal((n_test, d_in)) * 0.1).astype(np.float32)
-        clf = MLPClassifier(hidden_layer_sizes=hidden, random_state=1234, max_iter=8)
-        w = MLPWrapper(clf=clf)
-        import warnings
-        with warnings.catch_warnings():
-            warnings.simplefilter('ignore')
-            w.fit(X, Y)
-        probs = w.predict_probabilities(Xt)
-        assert clf.out_activation_ == 'logistic'
-        d = dict(X=Xt, probs=np.asarray(probs, dtype=np.float64), n_layers=np.int64(len(clf.coefs_)))
-        for i, (W, b) in enumerate(zip(clf.coefs_, clf.intercepts_)):
-            d[f'coef{i}'] = np.asarray(W, dtype=np.float32)
-            d[f'intercept{i}'] = np.asarray(b, dtype=np.float32)
-        np.savez_compressed(os.path.join(HERE, f'mlp_ref_{tag}.npz'), **d)
-        print('mlp', tag, probs.shape, float(probs.mean()))
+    # 'small': a fitted classifier, stored in full
+    d_in, hidden, n_labels, n_train, n_test = 24, (32, 16), 5, 200, 64
+    X = (rng.standard_normal((n_train, d_in)) * 0.1).astype(np.float32)
+    Y = (rng.random((n_train, n_labels)) < 0.2).astype(int)
+    Xt = (rng.standard_normal((n_test, d_in)) * 0.1).astype(np.float32)
+    clf = MLPClassifier(hidden_layer_sizes=hidden, random_state=1234, max_iter=8)
+    w = MLPWrapper(clf=clf)
+    with warnings.catch_warnings():
+        warnings.simplefilter('ignore')
+        w.fit(X, Y)
+    probs = w.predict_probabilities(Xt)
+    assert clf.out_activation_ == 'logistic'
+    d = dict(X=Xt, probs=np.asarray(probs, dtype=np.float64), n_layers=np.int64(len(clf.coefs_)))
+    for i, (W, b) in enumerate(zip(clf.coefs_, clf.intercepts_)):
+        d[f'coef{i}'] = np.asarray(W, dtype=np.float32)
+        d[f'intercept{i}'] = np.asarray(b, dtype=np.float32)
+    np.savez_compressed(os.path.join(HERE, 'mlp_ref_small.npz'), **d)
+    print('mlp small', probs.shape, float(probs.mean()))
+    # 'prod' (1600 -> 600 -> 600 -> 40): the weights alone would be 5 MB, so they and the inputs come from
+    # oracle.lstm_numpy.seeded_mlp; a classifier fitted for one step on a few rows supplies sklearn's attributes and
+    # then receives those weights, and the reference's wrapper computes the probabilities
+    dims, n_rows, seed = [1600, 600, 600, 40], 96, 4321
+    coefs, intercepts, Xt = seeded_mlp(seed, dims, n_rows)
+    clf = MLPClassifier(hidden_layer_sizes=tuple(dims[1:-1]), random_state=1234, max_iter=1)
+    w = MLPWrapper(clf=clf)
+    with warnings.catch_warnings():
+        warnings.simplefilter('ignore')
+        w.fit(Xt[:32], (rng.random((32, dims[-1])) < 0.2).astype(int))
+    clf.coefs_ = [c.astype(np.float64) for c in coefs]
+    clf.intercepts_ = [b.astype(np.float64) for b in intercepts]
+    probs = w.predict_probabilities(Xt)
+    assert clf.out_activation_ == 'logistic'
+    np.savez_compressed(os.path.join(HERE, 'mlp_ref_prod.npz'), seed=np.int64(seed), dims=np.array(dims, dtype=np.int64),
+                        n_rows=np.int64(n_rows), probs=np.asarray(probs, dtype=np.float64))
+    print('mlp prod', probs.shape, float(probs.mean()))
 
 
 def threshold_fixture():
@@ -85,7 +114,7 @@ def threshold_fixture():
     py/label_microservice/mlp.py:65-98) on preset scores: the classifier is a stand-in whose fit() does nothing and whose
     predict_proba() returns the preset score rows, so everything after `y_pred = ...` is the reference's code (with this
     image's sklearn precision_recall_curve).  Ties, a label without positives, labels that never qualify."""
-    sys.path.insert(0, '/root/reference/py')
+    sys.path.insert(0, os.path.join(reference_root(), 'py'))
     from label_microservice.mlp import MLPWrapper
     rng = np.random.default_rng(77)
     out = {}
@@ -154,10 +183,10 @@ def reference_driver_fixture():
             return types.SimpleNamespace(valid_dl=types.SimpleNamespace(x=types.SimpleNamespace(items=items)))
     sys.modules['fastai.text'].TextLMDataBunch = FakeLMDB
     torch.Tensor.cuda = lambda self, *a, **k: self
-    sys.path.insert(0, '/root/reference/py')
+    sys.path.insert(0, os.path.join(reference_root(), 'py'))
     from code_intelligence.inference import InferenceWrapper as RefWrapper
     import importlib.util
-    spec = importlib.util.spec_from_file_location('flask_app_inference', '/root/reference/Issue_Embeddings/flask_app/inference.py')
+    spec = importlib.util.spec_from_file_location('flask_app_inference', os.path.join(reference_root(), 'Issue_Embeddings/flask_app/inference.py'))
     fi = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(fi)          # the flask_app copy of the wrapper (df_to_emb, FI:136-212)
 
@@ -243,10 +272,10 @@ if __name__ == '__main__' and len(sys.argv) == 1:
     mlp_fixture()
 
 
-def full_size_fixture(name, n_layers, rows, T, seed, scale=1.0):
+def full_size_fixture(name, n_layers, rows, T, seed, scale=1.0, keep=None):
     """Reference-shape fixtures at the shapes bench.py / the sweep measure (weights re-derived from the seed).
-    rows: list of (count, min_len) groups; min_len None = fixed length T.  Stored compactly: int32 ids, f32 outputs,
-    plus the f64 per-row L2 norm of the oracle output (cheap sanity value for the loader)."""
+    rows: list of (count, min_len) groups; min_len None = fixed length T; keep: the row indices stored (every fixture
+    file stays under 1 MB).  Stored compactly: int32 ids, f32 outputs."""
     torch.set_num_threads(os.cpu_count())
     enc = R.make_encoder(seed, 60000, 800, 2400, n_layers, scale=scale)
     docs = []
@@ -259,14 +288,18 @@ def full_size_fixture(name, n_layers, rows, T, seed, scale=1.0):
         tt = int(lengths[b0:b0 + step].max())
         outs.append(R.encode_padded(enc, ids[b0:b0 + step, :tt], lengths[b0:b0 + step]))
     out = np.concatenate(outs).astype(np.float32)
+    if keep is not None:
+        ids, lengths, out = ids[keep], lengths[keep], out[keep]
     np.savez_compressed(os.path.join(HERE, name), cfg=np.array([n_layers, 800, 2400, 60000, seed], dtype=np.int64),
                         scale=np.float64(scale), ids=ids.astype(np.int32), lengths=lengths, expected=out)
     print(name, out.shape, float(np.abs(out).mean()), flush=True)
 
 
 def full_size():
-    # bench shape (BASELINE configs[1]): 256 x 512; rows 0..127 full length, rows 128..255 var-len in [64, 512]
-    full_size_fixture('encoder_r4_b256_t512.npz', 4, [(128, None), (128, 64)], 512, seed=1234)
+    # bench shape (BASELINE configs[1]): 256 x 512; rows 0..127 full length, rows 128..255 var-len in [64, 512]; stored:
+    # rows 0..31 and 128..143
+    full_size_fixture('encoder_r4_b256_t512.npz', 4, [(128, None), (128, 64)], 512, seed=1234,
+                      keep=np.r_[0:32, 128:144])
     # sweep buckets (configs[2]): lengths in (T/2, T]
     full_size_fixture('encoder_r4_t1024.npz', 4, [(32, 513)], 1024, seed=1234)
     full_size_fixture('encoder_r4_t2048.npz', 4, [(32, 1025)], 2048, seed=1234)

@@ -246,69 +246,71 @@ def test_bench_clock_sampler_summary():
     assert bench.ClockSampler.summarise([])["sm_mhz"] is None
 
 
-def _rot_schedule_model(T, ng, tiles, P, mma, lat, slots=2, pre=0.0):
-    """Event model of csrc/lstm_layer.cu's schedule: item n = t*C + g*tiles + j (C = ng*tiles) runs on CTA pair n % P, pairs
-    walk their items in increasing n; an item's MMAs start when the pair is free, every item of (t-1, g) has been
-    published (its MMA end + lat) and the pair's item `slots` positions back has left its TMEM slot (MMA end + lat).
-    `pre`: MMA time of the item that does NOT depend on (t-1, g) -- the fused input projection of the last layer (FUSE):
-    it starts as soon as the pair and the TMEM slot are free, only the remaining `mma` waits for the counter.
-    Returns (makespan, items seen, True if every dependency had a smaller index)."""
-    C, total = ng * tiles, T * ng * tiles
-    end, pub, cnt, tile_pub, pair_free = {}, {}, {}, {}, [0.0] * P
-    seen, ordered = set(), True
+def _rot_schedule_model(T, ng, tiles, P, mma, lat, epi=0.0, pre=0.0):
+    """Event model of csrc/lstm_layer.cu's schedule: item n = t*C + g*2*tiles + half*tiles + j (C = ng*2*tiles; timestep,
+    batch, 128-row half, column tile) runs on CTA n % P, and CTAs walk their items in increasing n.  An item's MMAs start
+    when its CTA has finished the previous item's epilogue (the accumulators live in the consumer warpgroups' registers)
+    and every item of (t-1, g) has been published (MMA + epilogue end + lat).  `pre`: MMA time of the part that does NOT
+    depend on (t-1, g) -- the fused input projection of the last layer (FUSE): it starts as soon as the CTA is free, only
+    `mma` waits for the counter.  Returns (makespan, items seen, True if every dependency had a smaller index)."""
+    per_batch = 2 * tiles
+    C, total = ng * per_batch, T * ng * per_batch
+    pub, cnt, tile_pub, cta_free = {}, {}, {}, [0.0] * P
+    seen, ordered, last = set(), True, 0.0
     for n in range(total):                      # ascending n is a valid evaluation order iff deps have smaller indices
-        p, k = n % P, n // P
+        p = n % P
         t, c = divmod(n, C)
-        g, j = divmod(c, tiles)
-        seen.add((t, g, j))
-        start = pair_free[p]
-        if k >= slots:
-            start = max(start, end[n - slots * P] + lat)
-        start += pre                            # the dependency-free part runs first
+        g, r = divmod(c, per_batch)
+        half, j = divmod(r, tiles)
+        seen.add((t, g, half, j))
+        start = cta_free[p] + pre               # the dependency-free part runs first
         if t > 0:
-            if (t - 1, g) not in pub:           # some tile of (t-1, g) has an index >= n: the order argument would break
+            if (t - 1, g) not in pub:           # some item of (t-1, g) has an index >= n: the order argument would break
                 ordered = False
                 break
             start = max(start, pub[(t - 1, g)])
-        end[n] = pair_free[p] = start + mma
-        tile_pub[(t, g)] = max(tile_pub.get((t, g), 0.0), end[n] + lat)
+        done = cta_free[p] = start + mma + epi
+        last = max(last, done)
+        tile_pub[(t, g)] = max(tile_pub.get((t, g), 0.0), done + lat)
         cnt[(t, g)] = cnt.get((t, g), 0) + 1
-        if cnt[(t, g)] == tiles:
+        if cnt[(t, g)] == per_batch:
             pub[(t, g)] = tile_pub[(t, g)]
-    return (max(end.values()) + lat if end else 0.0), len(seen), ordered
+    return last + lat, len(seen), ordered
 
 
 def test_rotating_schedule_model():
-    """Design claims of DESIGN.md section 4 / csrc/lstm_layer.cu, checked on a timing model: every (t, batch, tile) item is
-    dealt exactly once, an item only waits for smaller indices (=> no wait cycle for ANY pair count), and with five
-    batches at H = 2400 (C = 190 >= 2*74 + 38) the pairs issue back to back (within 2 % of 38*mma/74 per batch-step)
-    although each item's inputs take `lat` to become visible, while three batches leave that latency exposed."""
-    for (T, ng, tiles, P) in ((5, 1, 1, 74), (7, 3, 38, 74), (4, 5, 38, 74), (6, 5, 13, 74), (9, 2, 4, 3), (3, 5, 38, 1)):
-        span, n_items, ordered = _rot_schedule_model(T, ng, tiles, P, mma=1.0, lat=0.7)
-        assert ordered and n_items == T * ng * tiles and span > 0
-    mma, lat, T = 13.8, 8.0, 48
-    ideal = 38 * mma / 74
-    per_step = {ng: _rot_schedule_model(T, ng, 38, 74, mma, lat)[0] / T / ng for ng in (3, 5)}
+    """Design claims of DESIGN.md section 4 / csrc/lstm_layer.cu, checked on a timing model: every (t, batch, half, tile)
+    item is dealt exactly once, an item only waits for smaller indices (=> no wait cycle for ANY CTA count), and with five
+    batches at H = 2400 on the 132 SMs of an H100 (380 items per timestep) the CTAs work back to back (within 2 % of
+    76 (mma + epi) / 132 per batch-step) although each item's inputs take `lat` to become visible, while one batch leaves
+    that latency exposed.  Times in units of one k-block (38 per item)."""
+    for (T, ng, tiles, P) in ((5, 1, 1, 132), (7, 3, 38, 132), (4, 5, 38, 132), (6, 5, 13, 132), (9, 2, 4, 3), (3, 5, 38, 1)):
+        span, n_items, ordered = _rot_schedule_model(T, ng, tiles, P, mma=1.0, lat=0.7, epi=0.3)
+        assert ordered and n_items == T * ng * 2 * tiles and span > 0
+    mma, epi, lat, T = 38.0, 8.0, 20.0, 48
+    ideal = 76 * (mma + epi) / 132
+    per_step = {ng: _rot_schedule_model(T, ng, 38, 132, mma, lat, epi)[0] / T / ng for ng in (1, 5)}
     assert per_step[5] <= 1.02 * ideal, per_step
-    assert per_step[3] >= 1.15 * ideal, per_step          # 114 items per timestep: the dependency latency shows
+    assert per_step[1] >= 1.5 * ideal, per_step           # 76 items per timestep: the dependency latency shows
 
 
 def test_fused_last_layer_hides_its_step_chain_in_the_model():
     """Why the last layer's input projection rides its recurrent K loop (DESIGN.md section 4, csrc/lstm_layer.cu FUSE): with
-    13 tiles x 5 batches = 65 items per timestep on 74 pairs every pair has at most one item per timestep, so the hoisted
-    form is bound by the step chain (MMA + visibility latency per timestep) and the projection GEMM comes on top; with the
-    38 dependency-free k-blocks in front of the 13 recurrent ones the chain hides behind the item itself and the layer
-    runs at the rate of its MMA stream (65 / 74 of a pair per timestep).  Times in units of one k-block."""
-    T, ng, tiles, P = 64, 5, 13, 74
-    rec, pre, lat = 13.0, 38.0, 22.0          # k-blocks; visibility latency ~ epilogue + publish + counter + first tile
-    hoisted = _rot_schedule_model(T, ng, tiles, P, mma=rec, lat=lat)[0] / T
-    fused, n_items, ordered = _rot_schedule_model(T, ng, tiles, P, mma=rec, lat=lat, pre=pre)
+    13 tiles x 2 halves x 5 batches = 130 items per timestep on 132 CTAs every CTA has at most one item per timestep, so
+    the hoisted form is bound by the step chain (MMA + epilogue + visibility latency per timestep) and the projection GEMM
+    comes on top; with the 38 dependency-free k-blocks in front of the 13 recurrent ones the chain hides behind the item
+    itself and the layer runs at the rate of its MMA stream.  Times in units of one k-block."""
+    T, ng, tiles, P = 64, 5, 13, 132
+    rec, pre, epi, lat = 13.0, 38.0, 8.0, 20.0   # k-blocks; lat ~ publish + counter + first tile
+    hoisted = _rot_schedule_model(T, ng, tiles, P, mma=rec, lat=lat, epi=epi)[0] / T
+    fused, n_items, ordered = _rot_schedule_model(T, ng, tiles, P, mma=rec, lat=lat, epi=epi, pre=pre)
     fused /= T
-    assert ordered and n_items == T * ng * tiles
-    assert hoisted >= 0.95 * (rec + lat)                         # chain-bound: one MMA phase + one latency per timestep
-    gemm_equiv = pre * ng * tiles / P                            # the hoisted projection at full rate, per timestep
-    stream = (pre + rec) * ng * tiles / P                        # all 51 k-blocks of the 65 items on 74 pairs
-    assert fused <= 1.12 * stream, (fused, stream)               # MMA-stream-bound, chain hidden
+    assert ordered and n_items == T * ng * 2 * tiles
+    assert hoisted >= 0.95 * (rec + epi + lat)                   # chain-bound: one item + one latency per timestep
+    items = ng * 2 * tiles
+    gemm_equiv = pre * items / P                                 # the hoisted projection at full rate, per timestep
+    stream = (pre + rec + epi) * items / P                       # all work of the 130 items on 132 CTAs
+    assert fused <= 1.12 * stream, (fused, stream)               # stream-bound, chain hidden
     assert fused <= 0.80 * (hoisted + gemm_equiv), (fused, hoisted, gemm_equiv)
 
 

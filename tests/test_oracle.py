@@ -99,10 +99,8 @@ def test_batch_seq_pool_asserts_like_reference():
 @pytest.mark.parametrize("tag", ["small", "prod"])
 def test_mlp_numpy_restatement_matches_reference_fixture(golden_dir, tag):
     """mlp_ref_*.npz was produced by the reference's MLPWrapper.predict_probabilities."""
-    z = np.load(os.path.join(golden_dir, f"mlp_ref_{tag}.npz"))
-    n = int(z["n_layers"])
-    probs = N.mlp_forward(z["X"], [z[f"coef{i}"] for i in range(n)], [z[f"intercept{i}"] for i in range(n)])
-    np.testing.assert_allclose(probs, z["probs"], atol=2e-6)
+    coefs, intercepts, X, want = N.load_mlp_fixture(os.path.join(golden_dir, f"mlp_ref_{tag}.npz"))
+    np.testing.assert_allclose(N.mlp_forward(X, coefs, intercepts), want, atol=2e-6)
 
 
 def test_filter_labels_matches_reference_test_case():

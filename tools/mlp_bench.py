@@ -1,4 +1,4 @@
-"""BASELINE.json configs[4]: Label_Microservice head, 2400/1600-d -> (600,600) -> labels on 1xB200: rows/s, labels/s,
+"""BASELINE.json configs[4]: Label_Microservice head, 2400/1600-d -> (600,600) -> labels on one H100: rows/s, labels/s,
 max-abs probability difference and label-set agreement vs sklearn predict_proba (what MLPWrapper.predict_probabilities calls,
 py/label_microservice/mlp.py:63).  Prints one JSON line per input width."""
 import json, os, sys, time, warnings

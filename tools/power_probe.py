@@ -1,6 +1,6 @@
 """Development aid: board power / SM clock / achieved TFLOP/s of a workload run back to back for a few seconds, to
 compare energy per FLOP of the encoder paths with cuBLAS (the chip sits at its power cap under all of them,
-profiles/README.md "The kernel runs at the board's power cap").
+the kernels run at the board's power cap).
 
     python tools/power_probe.py --what cublas,enc,enc:IE_GX_BF16=0,enc256 --seconds 4 [--T 512]
 

@@ -1,7 +1,7 @@
 """BASELINE.json configs[2]: var-len bucketed sweep, seq_len 64..2048, bf16 tensor-core path vs the fp32 CPU oracle.
 Per bucket: 1280 issues (five batches of 256 per launch), lengths uniform in (T/2, T], right padded to T; parity of four
 rows against the live oracle (the full-size goldens of tests/golden cover 32..256 rows per shape in the test-suite).
-Prints one JSON line per bucket (copied to profiles/)."""
+Prints one JSON line per bucket."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

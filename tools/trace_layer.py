@@ -1,9 +1,8 @@
 """Development aid: per-item timeline of the persistent recurrent kernel (csrc/lstm_layer.cu).
 
-Slots per (cta, item k): 0 step counter seen by the h producer, 1 last h tile issued, 2 first h tile landed (MMA
-thread), 3 MMAs issued + commit, 4 accumulator seen by the epilogue, 5 epilogue stores done, 6 published, 7 c loaded;
-8/9/10/11 = SM cycles the MMA thread waited for h stages / W stages / spent from first stage to last issue / waited for
-the TMEM slot.  Times are %globaltimer ns.
+Slots the kernel writes per (cta, item k), %globaltimer ns: 0 step counter seen by the h producer, 1 last h tile
+issued, 2 first h_{t-1} stage landed (first consumer warpgroup), 3 that warpgroup's MMAs complete, 6 item published.
+The other slots of a record stay 0.
 """
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -13,7 +12,6 @@ from code_intelligence_b200 import IssueEncoder
 ap = argparse.ArgumentParser()
 ap.add_argument("--T", type=int, default=128)
 ap.add_argument("--layer", type=int, default=1)
-ap.add_argument("--ghz", type=float, default=1.9)
 ap.add_argument("--B", type=int, default=1280)
 ap.add_argument("--preroll", type=float, default=0.0, help="seconds of back-to-back encodes before the traced call (sustained clocks)")
 a = ap.parse_args()
@@ -48,59 +46,43 @@ else:
     enc.encode_ids(ids)
 ng = (a.B + 255) // 256
 tiles = 38 if a.layer < 3 else 13
-pairs = min(74, a.T * ng * tiles)
-items = (a.T * ng * tiles + pairs - 1) // pairs
-buf = np.zeros((2 * pairs, items, 12), dtype=np.int64)
+C = ng * 2 * tiles                          # items per timestep: batches x row halves x column tiles
+ctas = min(torch.cuda.get_device_properties(0).multi_processor_count, a.T * C)   # one item per CTA per round
+items = (a.T * C + ctas - 1) // ctas
+buf = np.zeros((ctas, items, 12), dtype=np.int64)
 n = enc._lib.ie_debug_seq_trace(enc._h, -1, buf.ctypes.data, buf.size)
-print("records", n, "pairs", pairs, "items/pair", items, "ng", ng, "tiles", tiles)
+print("records", n, "ctas", ctas, "items/cta", items, "ng", ng, "tiles", tiles)
 tr = buf.astype(np.float64)
-lead = tr[0::2]
 sel = slice(8, items - 3)
 us = 1e-3
-cyc = 1.0 / (a.ghz * 1e3)
-span = (lead[:, :, 6].max() - lead[:, 0, 0].min()) * us
+span = (tr[:, :, 6].max() - tr[:, 0, 0].min()) * us
 print(f"layer span {span / 1e3:.3f} ms = {span / a.T:.2f} us per timestep = {span / a.T / ng:.2f} us per batch-step")
-period = np.diff(lead[:, :, 3], axis=1)[:, sel] * us
-print(f"item period per pair (commit to commit): mean {period.mean():.2f} us  p10 {np.percentile(period, 10):.2f}  p90 {np.percentile(period, 90):.2f}")
-mma = (lead[:, :, 3] - lead[:, :, 2])[:, sel] * us
-print(f"MMA phase (first h landed -> commit): mean {mma.mean():.2f} us  max {mma.max():.2f}")
-idle = (lead[:, 1:, 2] - lead[:, :-1, 3])[:, sel] * us
-print(f"issuer idle between items (commit k -> first h of k+1 landed): mean {idle.mean():.2f} us  p90 {np.percentile(idle, 90):.2f}")
-flag_late = (lead[:, 1:, 0] - lead[:, :-1, 3])[:, sel] * us
-print(f"step counter of item k+1 seen relative to commit of item k: mean {flag_late.mean():.2f} us  p10 {np.percentile(flag_late, 10):.2f}  p90 {np.percentile(flag_late, 90):.2f}  (negative = early)")
-print(f"first h tile landed after counter seen: mean {((lead[:, :, 2] - lead[:, :, 0])[:, sel] * us).mean():.2f} us")
-print("MMA thread per item (us @%.2f GHz): waiting h stages %.2f, waiting W stages %.2f, first stage -> last issue %.2f, waiting TMEM slot %.2f" % (
-    a.ghz, lead[:, sel, 8].mean() * cyc, lead[:, sel, 9].mean() * cyc, lead[:, sel, 10].mean() * cyc, lead[:, sel, 11].mean() * cyc))
-ep = (tr[:, :, 5] - tr[:, :, 4])[:, sel] * us
-print(f"epilogue (accumulator seen -> stores done): mean {ep.mean():.2f} us max {ep.max():.2f}")
-print(f"epilogue waits for accumulator after c loaded: mean {((tr[:, :, 4] - tr[:, :, 7])[:, sel] * us).mean():.2f} us")
-pub = (tr[:, :, 6] - tr[:, :, 5])[:, sel] * us
-print(f"stores done -> published: mean {pub.mean():.2f} us")
+period = np.diff(tr[:, :, 6], axis=1)[:, sel] * us
+print(f"item period per CTA (publish to publish): mean {period.mean():.2f} us  p10 {np.percentile(period, 10):.2f}  p90 {np.percentile(period, 90):.2f}")
+mma = (tr[:, :, 3] - tr[:, :, 2])[:, sel] * us
+print(f"recurrent MMA phase (first h stage landed -> MMAs complete): mean {mma.mean():.2f} us  max {mma.max():.2f}")
+ep = (tr[:, :, 6] - tr[:, :, 3])[:, sel] * us
+print(f"epilogue + publish (MMAs complete -> published): mean {ep.mean():.2f} us  max {ep.max():.2f}")
+idle = (tr[:, 1:, 2] - tr[:, :-1, 6])[:, sel] * us
+print(f"published k -> first h stage of k+1 landed: mean {idle.mean():.2f} us  p90 {np.percentile(idle, 90):.2f}")
+print(f"first h stage landed after counter seen: mean {((tr[:, :, 2] - tr[:, :, 0])[:, sel] * us).mean():.2f} us")
 # dependency slack: item n needs every item of (t-1, g); when was the LAST of them published relative to our counter-seen time
-C = ng * tiles
-pub_t = np.full((a.T, ng), 0.0)
-for p in range(pairs):
+pub_t = np.zeros((a.T, ng))
+for p in range(ctas):
     for k in range(items):
-        nidx = p + k * pairs
+        nidx = p + k * ctas
         if nidx >= a.T * C:
             break
         t, c = divmod(nidx, C)
-        gidx = c // tiles
-        pub_t[t, gidx] = max(pub_t[t, gidx], tr[2 * p, k, 6], tr[2 * p + 1, k, 6])
+        pub_t[t, c // (2 * tiles)] = max(pub_t[t, c // (2 * tiles)], tr[p, k, 6])
 lat = []
-for p in range(0, pairs, 7):
+for p in range(0, ctas, 7):
     for k in range(8, items - 3):
-        nidx = p + k * pairs
+        nidx = p + k * ctas
         if nidx >= a.T * C:
             break
         t, c = divmod(nidx, C)
-        if t == 0:
-            continue
-        lat.append(lead[p, k, 0] - pub_t[t - 1, c // tiles])
+        if t > 0:
+            lat.append(tr[p, k, 0] - pub_t[t - 1, c // (2 * tiles)])
 lat = np.array(lat) * us
 print(f"counter seen after the last publish of (t-1, g): mean {lat.mean():.2f} us  p10 {np.percentile(lat, 10):.2f}  p90 {np.percentile(lat, 90):.2f}")
-for p in (0, 1, 36, pairs - 1):
-    r = lead[p]
-    rel = (r - r[:, 2:3]) * us
-    print(f"pair {p}: slots relative to first-h-landed (mean over items): " +
-          " ".join(f"{s}:{rel[sel, s].mean():+.2f}" for s in range(8)))

@@ -50,6 +50,10 @@ PROTOTYPES = {
                                    C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "ie_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                 C.c_void_p, C.c_int32]),
+    "ie_debug_gemm_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                   C.c_int32, C.c_int32, C.c_void_p, C.c_int32]),
+    "ie_debug_layer_states": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                                        C.c_void_p]),
 }
 
 _lib = None
@@ -81,6 +85,27 @@ def load() -> C.CDLL:
         fn.argtypes = args
     _lib = lib
     return lib
+
+
+def _debug_gemm(a, b, bias=None, act: int = 0, out_type: int = 0, segs: int = 1, device: int = 0):
+    """Test hook ``ie_debug_gemm_ex``: act(a [M,K] @ b [N,K]^T + bias) through the library's wgmma GEMM, stored as f32
+    (out_type 0), bf16 (1) or fp16 (2) and returned widened to float32 (M, N); segs 3 = split-bf16 operands."""
+    import numpy as np
+    a = np.ascontiguousarray(a, dtype=np.float32)
+    b = np.ascontiguousarray(b, dtype=np.float32)
+    (M, K), N = a.shape, b.shape[0]
+    if b.shape[1] != K:
+        raise ValueError(f"a {a.shape} and b {b.shape} disagree on K")
+    bias_p = None
+    if bias is not None:
+        bias = np.ascontiguousarray(bias, dtype=np.float32)
+        if bias.shape != (N,):
+            raise ValueError(f"bias {bias.shape} != ({N},)")
+        bias_p = bias.ctypes.data
+    d = np.empty((M, N), dtype=np.float32)
+    check(load().ie_debug_gemm_ex(a.ctypes.data, b.ctypes.data, bias_p, M, N, K, act, out_type, segs, d.ctypes.data,
+                                  device))
+    return d
 
 
 def check(rc: int) -> None:

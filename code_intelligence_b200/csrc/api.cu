@@ -9,6 +9,8 @@
 #include <string>
 #include <vector>
 
+#include <cuda_fp16.h>
+
 #include "../../include/issue_emb_b200.h"
 #include "kernels.h"
 
@@ -343,9 +345,10 @@ int check_persistent(ie_encoder* h, cudaStream_t s) {
   return IE_OK;
 }
 
-// the launch sequence shared by encode (pooled) and raw_features
+// the launch sequence shared by encode (pooled), raw_features and the layer-state hook: raw_out (optional) receives the
+// f32 hidden states of layer raw_layer as its recurrent kernel computed them, [B, T, out_l]
 int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B, int T, float* out, float* raw_out,
-                int flags, cudaStream_t s) {
+                int raw_layer, int flags, cudaStream_t s) {
   const ie_config& c = h->cfg;
   if (!h->emb_loaded) return fail(IE_ERR_STATE, "embedding not loaded");
   for (const Layer& L : h->layers)
@@ -353,6 +356,8 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
   if (B < 1 || B > h->max_batch) return fail(IE_ERR_INVALID, "B=%d outside [1,%d]", B, h->max_batch);
   if (T < 1) return fail(IE_ERR_INVALID, "T=%d must be >= 1", T);
   if (ids == nullptr || (out == nullptr && raw_out == nullptr)) return fail(IE_ERR_INVALID, "null pointer");
+  if (raw_out != nullptr && (raw_layer < 0 || raw_layer >= c.n_layers))
+    return fail(IE_ERR_INVALID, "layer %d out of range", raw_layer);
   const bool dev = (flags & IE_FLAG_DEVICE_PTRS) != 0;
   const bool pooled = out != nullptr;
   const int ng = (B + 255) / 256;
@@ -479,7 +484,7 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
       q.gx = from_table ? h->proj.p : h->gx.p;
       q.tok = from_table ? h->tok.as<int>() : nullptr;
       q.c = cstate; q.y = ybuf;
-      q.raw = (last && raw_out != nullptr) ? h->raw.as<float>() : nullptr;
+      q.raw = (l == raw_layer && raw_out != nullptr) ? h->raw.as<float>() : nullptr;
       q.pool_sum = (last && pooled) ? h->pool_sum.as<float>() : nullptr;
       q.pool_max = h->pool_max.as<float>(); q.pool_last = h->pool_last.as<float>();
       q.lengths = h->lengths.as<int>();
@@ -541,9 +546,10 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
       CK(cudaMemcpyAsync(out, out_dev, static_cast<size_t>(B) * 3 * c.emb_sz * sizeof(float), cudaMemcpyDeviceToHost, s));
   }
   if (raw_out != nullptr) {
-    // raw workspace is [b_pad, T, out_pad]; compact to [B, T, emb_sz]
-    CK(cudaMemcpy2DAsync(raw_out, static_cast<size_t>(c.emb_sz) * sizeof(float), h->raw.p,
-                         static_cast<size_t>(LL.out_pad) * sizeof(float), static_cast<size_t>(c.emb_sz) * sizeof(float),
+    // raw workspace is [b_pad, T, out_pad] of the requested layer; compact to [B, T, out]
+    const Layer& LR = h->layers[raw_layer];
+    CK(cudaMemcpy2DAsync(raw_out, static_cast<size_t>(LR.out) * sizeof(float), h->raw.p,
+                         static_cast<size_t>(LR.out_pad) * sizeof(float), static_cast<size_t>(LR.out) * sizeof(float),
                          static_cast<size_t>(B) * T, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s));
   }
   CK(cudaEventRecord(h->done_ev, s));
@@ -706,7 +712,7 @@ int ie_encoder_encode(ie_encoder* h, const int64_t* ids, const int32_t* lengths,
   // host-pointer mode: NULL selects the handle's own stream
   const bool dev = (flags & IE_FLAG_DEVICE_PTRS) != 0;
   cudaStream_t s = (stream || dev) ? static_cast<cudaStream_t>(stream) : h->own_stream;
-  int rc = run_encoder(h, ids, lengths, B, T, out, nullptr, flags, s);
+  int rc = run_encoder(h, ids, lengths, B, T, out, nullptr, -1, flags, s);
   if (rc != IE_OK || dev) return rc;
   return collect_errors(h);  // host-pointer mode: synchronous, device-side errors are reported by this call
 }
@@ -718,7 +724,19 @@ int ie_encoder_raw_features(ie_encoder* h, const int64_t* ids, int32_t B, int32_
   std::lock_guard<std::mutex> lk(h->mu);
   const bool dev = (flags & IE_FLAG_DEVICE_PTRS) != 0;
   cudaStream_t s = (stream || dev) ? static_cast<cudaStream_t>(stream) : h->own_stream;
-  int rc = run_encoder(h, ids, nullptr, B, T, nullptr, raw, flags, s);
+  int rc = run_encoder(h, ids, nullptr, B, T, nullptr, raw, h->cfg.n_layers - 1, flags, s);
+  if (rc != IE_OK || dev) return rc;
+  return collect_errors(h);
+}
+
+int ie_debug_layer_states(ie_encoder* h, int32_t layer, const int64_t* ids, int32_t B, int32_t T, float* out,
+                          int32_t flags, void* stream) {
+  if (h == nullptr) return fail(IE_ERR_INVALID, "null handle");
+  if (out == nullptr) return fail(IE_ERR_INVALID, "out is null");
+  std::lock_guard<std::mutex> lk(h->mu);
+  const bool dev = (flags & IE_FLAG_DEVICE_PTRS) != 0;
+  cudaStream_t s = (stream || dev) ? static_cast<cudaStream_t>(stream) : h->own_stream;
+  int rc = run_encoder(h, ids, nullptr, B, T, nullptr, out, layer, flags, s);
   if (rc != IE_OK || dev) return rc;
   return collect_errors(h);
 }
@@ -974,9 +992,11 @@ void ie_mlp_destroy(ie_mlp* m) {
   delete m;
 }
 
-int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
-                  float* d, int32_t device) {
+int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
+                     int32_t out_type, int32_t segs, float* d, int32_t device) {
   if (a == nullptr || b == nullptr || d == nullptr || M < 1 || N < 1 || K < 1) return fail(IE_ERR_INVALID, "bad argument");
+  if (act < 0 || act > 2 || out_type < 0 || out_type > 2 || (out_type == 2 && act != 0) || (segs != 1 && segs != 3))
+    return fail(IE_ERR_INVALID, "act=%d out_type=%d segs=%d not supported", act, out_type, segs);
   CK(cudaSetDevice(device));
   int sms = 132;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
@@ -987,17 +1007,21 @@ int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, 
   else if (n16 >= 128) bn = 128;
   else bn = n16;
   const int n_pad = static_cast<int>(round_up(N, bn));
+  // split-bf16 operands are [hi(k_pad) | lo(k_pad)] per row, as upload_sliced lays out the encoder's weights
+  const int ld = segs == 3 ? 2 * k_pad : k_pad;
+  const size_t elt = out_type == 0 ? 4 : 2;
   DevBuf fa, fb, ba, bb, dd, db;
   cudaStream_t s = nullptr;
   CK(fa.reserve(static_cast<size_t>(M) * K * 4));
   CK(fb.reserve(static_cast<size_t>(N) * K * 4));
-  CK(ba.reserve(static_cast<size_t>(m_pad) * k_pad * 2, true));
-  CK(bb.reserve(static_cast<size_t>(n_pad) * k_pad * 2, true));
-  CK(dd.reserve(static_cast<size_t>(m_pad) * n_pad * 4));
+  CK(ba.reserve(static_cast<size_t>(m_pad) * ld * 2, true));
+  CK(bb.reserve(static_cast<size_t>(n_pad) * ld * 2, true));
+  CK(dd.reserve(static_cast<size_t>(m_pad) * n_pad * elt));
   CK(cudaMemcpy(fa.p, a, static_cast<size_t>(M) * K * 4, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(fb.p, b, static_cast<size_t>(N) * K * 4, cudaMemcpyHostToDevice));
-  CK(ie::launch_convert_rows(fa.as<float>(), K, K, nullptr, M, ba.as<__nv_bfloat16>(), k_pad, 0, s));
-  CK(ie::launch_convert_rows(fb.as<float>(), K, K, nullptr, N, bb.as<__nv_bfloat16>(), k_pad, 0, s));
+  const int lo_off = segs == 3 ? k_pad : 0;
+  CK(ie::launch_convert_rows(fa.as<float>(), K, K, nullptr, M, ba.as<__nv_bfloat16>(), ld, lo_off, s));
+  CK(ie::launch_convert_rows(fb.as<float>(), K, K, nullptr, N, bb.as<__nv_bfloat16>(), ld, lo_off, s));
   if (bias) {
     std::vector<float> bp(n_pad, 0.0f);
     std::copy(bias, bias + N, bp.begin());
@@ -1005,17 +1029,38 @@ int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, 
     CK(cudaMemcpy(db.p, bp.data(), n_pad * 4, cudaMemcpyHostToDevice));
   }
   ie::GemmArgs g{};
-  g.a = ba.as<__nv_bfloat16>(); g.lda = k_pad;
-  g.b = bb.as<__nv_bfloat16>(); g.ldb = k_pad;
+  g.a = ba.as<__nv_bfloat16>(); g.lda = ld;
+  g.b = bb.as<__nv_bfloat16>(); g.ldb = ld;
   g.d = dd.p; g.ldd = n_pad;
   g.bias = bias ? db.as<float>() : nullptr;
   g.m_pad = m_pad; g.n_pad = n_pad; g.k_pad = k_pad;
-  g.m_store = M; g.n_store = n_pad; g.bn = bn; g.act = act; g.out_bf16 = 0; g.num_sms = sms;
+  g.m_store = M; g.n_store = n_pad; g.bn = bn; g.act = act; g.out_bf16 = out_type; g.num_sms = sms; g.segs = segs;
   CK(ie::launch_gemm_bf16(g, s));
-  CK(cudaMemcpy2D(d, static_cast<size_t>(N) * 4, dd.p, static_cast<size_t>(n_pad) * 4, static_cast<size_t>(N) * 4, M,
-                  cudaMemcpyDeviceToHost));
-  fa.release(); fb.release(); ba.release(); bb.release(); dd.release(); db.release();
+  if (out_type == 0) {
+    CK(cudaMemcpy2D(d, static_cast<size_t>(N) * 4, dd.p, static_cast<size_t>(n_pad) * 4, static_cast<size_t>(N) * 4, M,
+                    cudaMemcpyDeviceToHost));
+  } else {
+    // 16-bit results widened exactly to f32 on the host
+    std::vector<uint16_t> h16(static_cast<size_t>(M) * N);
+    CK(cudaMemcpy2D(h16.data(), static_cast<size_t>(N) * 2, dd.p, static_cast<size_t>(n_pad) * 2, static_cast<size_t>(N) * 2,
+                    M, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < h16.size(); ++i) {
+      if (out_type == 1) {
+        const uint32_t bits = static_cast<uint32_t>(h16[i]) << 16;
+        std::memcpy(d + i, &bits, 4);
+      } else {
+        __half_raw r;
+        r.x = h16[i];
+        d[i] = __half2float(__half(r));
+      }
+    }
+  }
   return IE_OK;
+}
+
+int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
+                  float* d, int32_t device) {
+  return ie_debug_gemm_ex(a, b, bias, M, N, K, act, 0, 1, d, device);
 }
 
 }  // extern "C"

@@ -156,6 +156,22 @@ class IssueEncoder:
         check(self._lib.ie_encoder_raw_features(self._h, ids.ctypes.data, B, T, raw.ctypes.data, 0, None))
         return raw
 
+    def _debug_layer_states(self, layer: int, ids) -> np.ndarray:
+        """Test hook ``ie_debug_layer_states``: hidden states of ``layer`` (B, T, out_l) float32 as its recurrent kernel
+        computed them (the ring holds their bf16 rounding); for the last layer identical to ``raw_features``."""
+        ids = np.ascontiguousarray(np.asarray(ids.cpu() if hasattr(ids, "cpu") else ids), dtype=np.int64)
+        if ids.ndim != 2:
+            raise ValueError("ids must be (B, T)")
+        B, T = ids.shape
+        if B > self.max_batch:
+            raise ValueError(f"B={B} > {self.max_batch}")
+        if not 0 <= layer < self.n_layers:
+            raise ValueError(f"layer {layer} outside [0, {self.n_layers})")
+        out_l = self.emb_sz if layer == self.n_layers - 1 else self.n_hid
+        out = np.empty((B, T, out_l), dtype=np.float32)
+        check(self._lib.ie_debug_layer_states(self._h, layer, ids.ctypes.data, B, T, out.ctypes.data, 0, None))
+        return out
+
     @property
     def max_batch(self) -> int:
         """Rows one C-ABI encode call takes: 256 x batches per launch (1280 by default, IE_BATCHES=n changes it)."""

@@ -53,8 +53,8 @@ extern "C" {
 
 #define IE_MAX_BATCH 3072 /* upper bound of rows per ie_encoder_encode call; the handle's own limit is
                              ie_encoder_max_batch() = 256 x (batches per launch, default 5): that many independent
-                             256-row batches ride one launch of the persistent recurrent kernel (each a CTA-pair
-                             M=256 UMMA tile); they share the kernel, not their results */
+                             256-row batches ride one launch of the persistent recurrent kernel (each as two 128-row
+                             halves of wgmma items); they share the kernel, not their results */
 
 typedef struct ie_encoder ie_encoder;
 typedef struct ie_mlp ie_mlp;
@@ -97,7 +97,7 @@ int ie_encoder_load_layer(ie_encoder* h, int32_t layer, const float* w_ih, const
  *   lengths [B] int32, 1 <= lengths[b] <= T
  *   out     [B, 3*emb_sz] f32 = [mean | max | last] over the first lengths[b] steps of the last layer's hidden
  *           states, zero initial state (encoder.reset(), inference.py:56)
- * 1 <= B <= ie_encoder_max_batch(h).  T is bounded only by the workspace cap B_pad*T <= 2^22 tokens (IE_ERR_OOM
+ * 1 <= B <= ie_encoder_max_batch(h).  T is bounded only by the workspace cap B_pad*T <= 2^27 tokens (IE_ERR_OOM
  * beyond; B_pad = B rounded up to 256): the time dimension is processed in chunks, so a single 16k-token issue is
  * fine. */
 int ie_encoder_encode(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int32_t B, int32_t T, float* out,
@@ -154,10 +154,26 @@ int ie_pr_thresholds(const float* scores, const uint8_t* truth, int32_t n, int32
                      double recall_threshold, float* thresholds, double* precisions, double* recalls, int32_t device,
                      int32_t flags, void* stream);
 
-/* Debug / test hook: D[M,N] = A[M,K] * B[N,K]^T (+bias) through the same wgmma GEMM the encoder uses.
- * a [M,K], b [N,K], bias [N] or NULL: host f32 (rounded to bf16 on the device); d [M,N] host f32. */
+/* Debug / test hook: D[M,N] = act(A[M,K] * B[N,K]^T (+bias)) through the same wgmma GEMM the encoder uses.
+ * a [M,K], b [N,K], bias [N] or NULL: host f32 (rounded to bf16 on the device); d [M,N] host f32;
+ * act 0 none, 1 relu, 2 sigmoid. */
 int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
                   float* d, int32_t device);
+
+/* Same GEMM with every epilogue and operand form the library uses: out_type 0 = f32, 1 = bf16 (the MLP head's hidden
+ * layers), 2 = fp16 (the encoder's input projections and per-token table; act must be 0), each widened exactly to f32
+ * into d; segs 1 = bf16 operands, 3 = split-bf16 (x = hi + lo, hi = bf16(x), lo = bf16(x - hi), products
+ * hi*hi + lo*hi + hi*lo: the fp32-accurate mode's operands). */
+int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
+                     int32_t out_type, int32_t segs, float* d, int32_t device);
+
+/* Debug / test hook: the hidden states of layer `layer` of an encode of ids [B, T] (zero initial state), as that
+ * layer's recurrent kernel computed them: out [B, T, out_l] f32, out_l = n_hid, or emb_sz for the last layer.  The
+ * hidden-state ring the next step and the next layer read holds their bf16 round-to-nearest-even (hi + lo in the
+ * fp32-accurate mode); for the last layer they are ie_encoder_raw_features.  Every development knob applies as in
+ * ie_encoder_encode; the arithmetic is the same, only an extra f32 store of h is made. */
+int ie_debug_layer_states(ie_encoder* h, int32_t layer, const int64_t* ids, int32_t B, int32_t T, float* out,
+                          int32_t flags, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,0 +1,117 @@
+"""CPU self-tests of oracle/device_numerics.py, the device-precision reference of tests/test_gpu_numerics.py: with every
+rounding switched off it is the plain LSTM; the teacher-forced prediction of a free-running float32 emulation of the
+device lies inside its own bound; each mutant of the arithmetic breaks that bound on the same data."""
+from dataclasses import replace
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import awd_lstm_ref as R
+from oracle import device_numerics as D
+from oracle import lstm_numpy as N
+
+CFG = (3, 96, 200, 500)
+
+
+@pytest.fixture(scope="module")
+def small():
+    ref = R.make_encoder(7, CFG[3], CFG[1], CFG[2], CFG[0], scale=2.0)
+    emb, layers = ref.export_weights()
+    ids = np.stack(R.synthetic_ids(32, 33, seed=3, vocab_sz=CFG[3]))
+    return emb, layers, ids
+
+
+def _mutant(mode, layer, name):
+    if name == "gx_bf16":
+        return replace(mode, gx="bf16") if mode.gx in ("fp16", "f32") else mode
+    if name == "cell_bf16":
+        return replace(mode, cell="bf16")
+    if name == "stale_c":
+        return replace(mode, stale_c=(0, 1, 2, 3)) if layer == 0 else mode
+    if name == "swap_fo":
+        return replace(mode, swap_fo=(0,)) if layer == 1 else mode
+    return mode
+
+
+def _teacher_forced(emb, layers, ids, states, modes, mutant=None):
+    xs = [emb[ids]] + states[:-1]
+    stats = [D.ratio_stats(states[l], *D.teacher_forced_layer(xs[l], states[l], layers[l], _mutant(modes[l], l, mutant)))
+             for l in range(len(layers))]
+    return max(s["max"] for s in stats), max(s["rms"] for s in stats)
+
+
+def test_without_rounding_it_is_the_plain_lstm(small):
+    emb, layers, ids = small
+    states = D.free_run(emb, layers, ids, [D.EXACT] * len(layers), torch.float64)
+    _, want = N.encode(emb, layers, ids, [ids.shape[1]] * len(ids))
+    np.testing.assert_allclose(states[-1].numpy(), want, rtol=0, atol=1e-12)
+    # teacher forcing on exact data with exact arithmetic predicts it exactly (bound 0)
+    pred, bound = D.teacher_forced_layer(emb[ids], states[0], layers[0], D.EXACT)
+    np.testing.assert_allclose(pred.numpy(), states[0].numpy(), rtol=0, atol=1e-12)
+    assert float(bound.max()) == 0.0
+
+
+@pytest.mark.parametrize("flags,env", [(0, None), (0, {"IE_FAST_MATH": 0}), (0, {"IE_GX_BF16": 0}),
+                                       (0, {"IE_FUSE_LAST": 0}), (D.IE_CFG_FP32, None)])
+def test_free_running_emulation_inside_bound_and_mutants_outside(small, flags, env):
+    """Observed here (float32 emulation, torch gates): design max ratio 0.43 (default) to 0.98 (IEEE-like gates), every
+    mutant's max ratio >= 7.8 and its RMS ratio >= 1.7, i.e. at least 8x beyond the design."""
+    emb, layers, ids = small
+    modes = D.layer_modes(len(layers), flags, env)
+    states = D.free_run(emb, layers, ids, modes, torch.float32)
+    mx, rms = _teacher_forced(emb, layers, ids, states, modes)
+    assert mx <= 1.0 and rms <= 0.05, (mx, rms)
+    for name in ("gx_bf16", "cell_bf16", "stale_c", "swap_fo"):
+        m_mx, m_rms = _teacher_forced(emb, layers, ids, states, modes, name)
+        assert m_mx > 4.0 or m_rms > 1.0, (name, m_mx, m_rms)
+
+
+def test_layer_modes_follow_the_knobs():
+    assert [m.gx for m in D.layer_modes(4)] == ["fp16", "fp16", "fp16", "fused"]
+    assert [m.gx for m in D.layer_modes(4, 0, {"IE_SEQ": 0})] == ["fp16"] * 4
+    assert [m.gx for m in D.layer_modes(3, 0, {"IE_GX_BF16": 0})] == ["f32", "f32", "fused"]
+    fp32 = D.layer_modes(3, D.IE_CFG_FP32, {"IE_GX_BF16": 1, "IE_FAST_MATH": 1})
+    assert all(m.segs == 3 and m.gx == "f32" and m.gates == "ieee" for m in fp32)
+    assert D.layer_modes(2, D.IE_CFG_ACCURATE_GATES)[0].gates == "exp"
+
+
+def test_pool_restates_the_kernel_and_mutants_differ():
+    rng = np.random.default_rng(0)
+    h = (rng.standard_normal((6, 9, 5)) * 0.3).astype(np.float32)
+    lengths = np.array([1, 4, 5, 9, 2, 7])
+    got = D.pool(h, lengths)
+    for b, n in enumerate(lengths):
+        s = h[b, 0].copy()
+        for t in range(1, n):
+            s = (s + h[b, t]).astype(np.float32)
+        np.testing.assert_array_equal(got[b, :5], s * (np.float32(1) / np.float32(n)))
+        np.testing.assert_array_equal(got[b, 5:10], h[b, :n].max(0))
+        np.testing.assert_array_equal(got[b, 10:], h[b, n - 1])
+    assert not np.array_equal(D.pool(h, lengths, "ring"), got)
+    assert not np.array_equal(D.pool(h, lengths, "max_pad"), got)
+
+
+def test_gemm_interval_and_mlp_head_contain_float32_emulations():
+    rng = np.random.default_rng(1)
+    a = rng.standard_normal((40, 300)).astype(np.float32)
+    b = (rng.standard_normal((24, 300)) / np.sqrt(300)).astype(np.float32)
+    bias = rng.standard_normal(24).astype(np.float32)
+    ab, bb = (torch.from_numpy(v).bfloat16().float() for v in (a, b))
+    z32 = ab @ bb.T + torch.from_numpy(bias)
+    for act, out, f in ((0, "fp16", lambda z: z.half()), (1, "bf16", lambda z: z.clamp_min(0).bfloat16()),
+                        (2, "f32", torch.sigmoid)):
+        lo, hi, _ = D.gemm_interval(a, b, bias, act, out, 1)
+        d = f(z32).double()
+        assert bool(((d >= lo) & (d <= hi)).all()), (act, out)
+    lo3, hi3, _ = D.gemm_interval(a, b, None, 0, "f32", 3)
+    d1 = (ab @ bb.T).double()                      # bf16 operands break the split-bf16 bound on most elements
+    assert float(((d1 < lo3) | (d1 > hi3)).double().mean()) > 0.5
+    coefs = [rng.uniform(-0.1, 0.1, (300, 64)).astype(np.float32), rng.uniform(-0.2, 0.2, (64, 7)).astype(np.float32)]
+    ints = [rng.uniform(-0.1, 0.1, 64).astype(np.float32), rng.uniform(-1, 0, 7).astype(np.float32)]
+    x = torch.from_numpy(a).bfloat16().float()
+    hdn = (x @ torch.from_numpy(coefs[0]).bfloat16().float() + torch.from_numpy(ints[0])).clamp_min(0).bfloat16().float()
+    p32 = torch.sigmoid(hdn @ torch.from_numpy(coefs[1]).bfloat16().float() + torch.from_numpy(ints[1])).double()
+    _, lo, hi = D.mlp_head(a, coefs, ints)
+    assert bool(((p32 >= lo) & (p32 <= hi)).all())
+    np.testing.assert_allclose(D.mlp_head(a, coefs, ints)[0].numpy(), N.mlp_forward(a, coefs, ints), atol=5e-3)

@@ -1,6 +1,7 @@
 // C-ABI layer of libissue_emb_b200.so (declared in include/issue_emb_b200.h): handle management, weight
 // re-layout, workspace, and the launch sequence of the encoder hot path and the MLP head.
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -964,8 +965,12 @@ int ie_pr_thresholds(const float* scores, const uint8_t* truth, int32_t n, int32
                                 recalls, s));
     return IE_OK;
   }
-  DevBuf ds, dt, dth, dp, dr;
   const size_t cells = static_cast<size_t>(n) * n_labels;
+  for (size_t i = 0; i < cells; ++i)   // sklearn's precision_recall_curve raises on NaN / inf
+    if (!std::isfinite(scores[i]))
+      return fail(IE_ERR_INVALID, "scores[%zu][%zu] = %g is not finite", i / n_labels, i % n_labels,
+                  static_cast<double>(scores[i]));
+  DevBuf ds, dt, dth, dp, dr;
   CK(ds.reserve(cells * sizeof(float)));
   CK(dt.reserve(cells));
   CK(dth.reserve(n_labels * sizeof(float)));

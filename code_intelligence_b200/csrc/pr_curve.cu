@@ -12,6 +12,11 @@
 // (order-preserving score encoding in the high word), bitonic-sorted descending, the truth bits are prefix-summed, and
 // every position that ends a group of equal scores is a curve point.  n <= 16384 samples per call (128 KB of keys);
 // larger hold-out sets stay on the host path.
+//
+// Input domain: finite scores.  -0.0 and +0.0 are one score (sklearn groups them, np.diff of the two is 0), so zero is
+// canonicalised before encoding.  sklearn raises on NaN / inf; a device-pointer call cannot return an error, so a label
+// with any non-finite score gets threshold, precision and recall NaN (an excluded label gets NaN / 0 / 0).  The host
+// entry point rejects such scores before anything is launched.
 #include "kernels.h"
 #include "lstm_common.cuh"
 
@@ -31,16 +36,27 @@ pr_threshold_kernel(const float* __restrict__ scores, const uint8_t* __restrict_
   __shared__ int best_idx[32];
   const int label = blockIdx.x;
   const int tid = threadIdx.x;
+  int nonfinite = 0;
   for (int i = tid; i < n_pow2; i += kPrThreads) {
     unsigned long long k = 0ull;   // padding sorts to the end (real keys have the high word >= 1: enc_max(x) > 0 for finite x)
     if (i < n) {
-      const float s = scores[static_cast<long long>(i) * n_labels + label];
+      float s = scores[static_cast<long long>(i) * n_labels + label];
+      nonfinite |= !isfinite(s);
+      s = (s == 0.0f) ? 0.0f : s;   // -0.0 -> +0.0: one tie group, as in sklearn
       const unsigned t = truth[static_cast<long long>(i) * n_labels + label] ? 1u : 0u;
       k = (static_cast<unsigned long long>(enc_max(s)) << 32) | t;
     }
     keys[i] = k;
   }
-  __syncthreads();
+  if (__syncthreads_or(nonfinite)) {   // uniform across the CTA
+    if (tid == 0) {
+      const float qnan = __int_as_float(0x7fc00000);
+      out_thr[label] = qnan;
+      out_prec[label] = static_cast<double>(qnan);
+      out_rec[label] = static_cast<double>(qnan);
+    }
+    return;
+  }
   // bitonic sort, descending
   for (int size = 2; size <= n_pow2; size <<= 1) {
     for (int stride = size >> 1; stride > 0; stride >>= 1) {

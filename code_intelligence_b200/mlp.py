@@ -41,9 +41,12 @@ def pr_thresholds_host(scores, truth, precision_threshold, recall_threshold):
 
 
 def pr_thresholds(scores, truth, precision_threshold, recall_threshold, device: int = 0):
-    """Same on the GPU (``ie_pr_thresholds``, csrc/pr_curve.cu): scores (n, L) float32, truth (n, L) 0/1, n <= 16384."""
-    lib = _lib.load()
+    """Same on the GPU (``ie_pr_thresholds``, csrc/pr_curve.cu): scores (n, L) float32, truth (n, L) 0/1, n <= 16384.
+    Raises ValueError on NaN or infinite scores, as sklearn's precision_recall_curve does."""
     scores = np.ascontiguousarray(scores, dtype=np.float32)
+    if not np.isfinite(scores).all():
+        raise ValueError("scores contain NaN or infinity")
+    lib = _lib.load()
     truth = np.ascontiguousarray(np.asarray(truth) != 0, dtype=np.uint8)
     n, L = scores.shape
     assert truth.shape == (n, L)
@@ -145,10 +148,14 @@ class MLPWrapper:
         self._head = None
 
     def predict_probabilities(self, X):
-        """Predict probabilities of all labels for data -> (n_samples, n_classes); on the H100."""
+        """Predict probabilities of all labels for data -> (n_samples, n_classes); on the H100.  Like sklearn's
+        predict_proba, a network with one output unit (one label column, or a 1-D y) gives (n, 2) = [1 - p, p]."""
         if self._head is None:
             self._head = MLPHead.from_sklearn(self.clf, self._device)
-        return self._head.predict_proba(X)
+        p = self._head.predict_proba(X)
+        if p.shape[1] == 1:
+            return np.hstack([1.0 - p, p])
+        return p
 
     def find_probability_thresholds(self, X, y, test_size=0.3):
         """mlp.py:65-98: hold out ``test_size`` of the data (random_state 1234), fit on the rest, and for every label keep
@@ -160,9 +167,11 @@ class MLPWrapper:
         from sklearn.model_selection import train_test_split
         X_train, X_test, y_train, y_test = train_test_split(X, y, test_size=test_size, random_state=1234)
         self.fit(X_train, y_train)
-        scores = self.predict_probabilities(X_test)
         truth = np.asarray(y_test)
         self.total_labels_count = truth.shape[1]
+        # label l is scored by column l, as the reference indexes y_pred[:, label]: with one label column that is the
+        # [1 - p, p] head's column 0
+        scores = self.predict_probabilities(X_test)[:, :self.total_labels_count]
         if truth.shape[0] <= PR_MAX_SAMPLES:
             thr, prec, rec = pr_thresholds(scores, truth, self.precision_threshold, self.recall_threshold, self._device)
         else:

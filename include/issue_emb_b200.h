@@ -149,7 +149,10 @@ void ie_mlp_destroy(ie_mlp* m);
  *   scores [n, n_labels] f32 (predict_proba of the hold-out set), truth [n, n_labels] uint8 (0/1), n <= 16384
  *   thresholds [n_labels] f32 (NaN: no qualifying point, the label is excluded -- None in the reference),
  *   precisions / recalls [n_labels] f64 at the chosen point (0 when excluded).
- * Host pointers (synchronous) or, with IE_FLAG_DEVICE_PTRS, device pointers on `device` (asynchronous on `stream`). */
+ * Scores must be finite; -0.0 and +0.0 are the same score (a zero threshold is returned as +0.0).
+ * Host pointers (synchronous; a NaN or infinite score returns IE_ERR_INVALID before anything is launched) or, with
+ * IE_FLAG_DEVICE_PTRS, device pointers on `device` (asynchronous on `stream`; a label with any NaN or infinite score
+ * gets threshold, precision and recall all NaN, which an excluded label -- NaN / 0 / 0 -- never has). */
 int ie_pr_thresholds(const float* scores, const uint8_t* truth, int32_t n, int32_t n_labels, double precision_threshold,
                      double recall_threshold, float* thresholds, double* precisions, double* recalls, int32_t device,
                      int32_t flags, void* stream);

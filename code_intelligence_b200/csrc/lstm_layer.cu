@@ -31,6 +31,8 @@
 // either gets the whole grid resident or fails; a wait that still exceeds its limit raises the abort protocol of ptx.cuh.
 #include <cmath>
 
+#include <type_traits>
+
 #include <cuda_fp16.h>
 
 #include "kernels.h"
@@ -48,6 +50,10 @@ constexpr int kLRows = 128;             // batch rows per item
 constexpr uint32_t kHBytes = kLRows * 64 * 2;
 constexpr uint32_t kWBytes = kLTileN * 64 * 2;
 constexpr uint32_t kStageBytes = kHBytes + kWBytes;
+// units of the epilogue whose loads are in flight together (divides 16).  Larger groups spill: the consumers already
+// hold 128 accumulators within the 168 registers a thread has at 384 threads per SM
+constexpr int kEpiGroup = 2;
+static_assert(16 % kEpiGroup == 0, "kEpiGroup must divide 16");
 
 __device__ __forceinline__ void st_release_cta(uint32_t* p, uint32_t v) {
   asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
@@ -292,34 +298,55 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
         __nv_bfloat16* yrow = a.y + (static_cast<long long>(t + 1) * b_pad + brow) * a.ldy + unit0;
         const long long po = static_cast<long long>(brow) * a.out_pad + unit0;
         const long long gbase = grow * (4ll * a.out_pad) + j * kLTileN + 2 * q;
+        // the 16 units run in groups of kEpiGroup: a group's loads (Gx or bias, c_{t-1}) are all issued before its
+        // stores, so their latencies overlap -- loads after the previous unit's stores would be a chain of 32
+        // dependent L2 / HBM round trips per item (the compiler cannot move a load above a store it may alias)
 #pragma unroll
-        for (int m = 0; m < 16; ++m) {
+        for (int m0 = 0; m0 < 16; m0 += kEpiGroup) {
           // this thread's unit 4m+q of the tile: (i, f) at columns 16m + 2q (+1), (g, o) at 16m + 8 + 2q (+1)
-          float2 gif, ggo;
-          if constexpr (FUSE) {
-            gif = __ldg(reinterpret_cast<const float2*>(a.bias + j * kLTileN + 2 * q + 16 * m));
-            ggo = __ldg(reinterpret_cast<const float2*>(a.bias + j * kLTileN + 2 * q + 16 * m + 8));
-          } else if constexpr (GXBF) {
-            const __half2* gp = reinterpret_cast<const __half2*>(reinterpret_cast<const __half*>(a.gx) + gbase + 16 * m);
-            gif = __half22float2(__ldcs(gp));
-            ggo = __half22float2(__ldcs(gp + 4));
-          } else {
-            const float2* gp = reinterpret_cast<const float2*>(reinterpret_cast<const float*>(a.gx) + gbase + 16 * m);
-            gif = __ldcs(gp);
-            ggo = __ldcs(gp + 4);
+          using GxT = typename std::conditional<GXBF && !FUSE, __half2, float2>::type;
+          GxT gif[kEpiGroup], ggo[kEpiGroup];
+          float cprev[kEpiGroup];
+#pragma unroll
+          for (int i = 0; i < kEpiGroup; ++i) {
+            const int m = m0 + i;
+            if constexpr (FUSE) {
+              gif[i] = __ldg(reinterpret_cast<const float2*>(a.bias + j * kLTileN + 2 * q + 16 * m));
+              ggo[i] = __ldg(reinterpret_cast<const float2*>(a.bias + j * kLTileN + 2 * q + 16 * m + 8));
+            } else if constexpr (GXBF) {
+              const __half2* gp = reinterpret_cast<const __half2*>(reinterpret_cast<const __half*>(a.gx) + gbase + 16 * m);
+              gif[i] = __ldcs(gp);
+              ggo[i] = __ldcs(gp + 4);
+            } else {
+              const float2* gp = reinterpret_cast<const float2*>(reinterpret_cast<const float*>(a.gx) + gbase + 16 * m);
+              gif[i] = __ldcs(gp);
+              ggo[i] = __ldcs(gp + 4);
+            }
+            cprev[i] = (tg == 0) ? 0.0f : __ldcg(cp + 4 * m);
           }
-          const float zi = d[8 * m + 2 * hr] + gif.x;
-          const float zf = d[8 * m + 2 * hr + 1] + gif.y;
-          const float zg = d[8 * m + 4 + 2 * hr] + ggo.x;
-          const float zo = d[8 * m + 4 + 2 * hr + 1] + ggo.y;
-          const float cprev = (tg == 0) ? 0.0f : __ldcg(cp + 4 * m);
-          float cnew, hn;
-          lstm_cell1(zi, zf, zg, zo, cprev, cnew, hn, a.gate_mode);
-          __stcg(cp + 4 * m, cnew);
-          store_h1(yrow + 4 * m, hn, lo_off);
-          if (a.raw != nullptr)
-            a.raw[(static_cast<long long>(brow) * a.T_total + tg) * a.raw_ld + unit0 + 4 * m] = hn;
-          if constexpr (POOL) pool_accumulate1(a.pool_sum, a.pool_max, a.pool_last, po + 4 * m, hn, tg, len);
+#pragma unroll
+          for (int i = 0; i < kEpiGroup; ++i) {
+            const int m = m0 + i;
+            float2 gi, go;
+            if constexpr (GXBF && !FUSE) {
+              gi = __half22float2(gif[i]);
+              go = __half22float2(ggo[i]);
+            } else {
+              gi = gif[i];
+              go = ggo[i];
+            }
+            const float zi = d[8 * m + 2 * hr] + gi.x;
+            const float zf = d[8 * m + 2 * hr + 1] + gi.y;
+            const float zg = d[8 * m + 4 + 2 * hr] + go.x;
+            const float zo = d[8 * m + 4 + 2 * hr + 1] + go.y;
+            float cnew, hn;
+            lstm_cell1(zi, zf, zg, zo, cprev[i], cnew, hn, a.gate_mode);
+            __stcg(cp + 4 * m, cnew);
+            store_h1(yrow + 4 * m, hn, lo_off);
+            if (a.raw != nullptr)
+              a.raw[(static_cast<long long>(brow) * a.T_total + tg) * a.raw_ld + unit0 + 4 * m] = hn;
+            if constexpr (POOL) pool_accumulate1(a.pool_sum, a.pool_max, a.pool_last, po + 4 * m, hn, tg, len);
+          }
         }
       }
       // publish (step t, batch g): h_t / c_t / pooling state visible

@@ -22,22 +22,34 @@ def small():
     return emb, layers, ids
 
 
-def _mutant(mode, layer, name):
+# the shape classes of tests/test_gpu_config_space.py: one layer, emb_sz > n_hid, width 1 (vocab 500 rather than the
+# smallest model's 3: three tokens give layer 0 three distinct inputs, too few for a per-element statistic)
+SHAPES = {"1 layer": (1, 96, 8, 500), "emb > hid": (3, 200, 96, 500), "width 1": (2, 1, 1, 500)}
+# Mutants that exceed the bound, but by less than 4x.  At one unit the weights and the bias are O(1) (torch init
+# U(+-1/sqrt(H))), so the tanh.approx allowance (2^-11 relative) in the bound is as large as the bf16 rounding of Gx or
+# of the cell state: max ratio 1.7-1.8 (gx_bf16) and 3.3 (cell_bf16) with fast gates, against a design max of 0.0001.
+WEAK = {("width 1", "gx_bf16", "fast"), ("width 1", "cell_bf16", "fast")}
+
+
+def _mutant(mode, layer, name, n_layers, width):
     if name == "gx_bf16":
         return replace(mode, gx="bf16") if mode.gx in ("fp16", "f32") else mode
     if name == "cell_bf16":
         return replace(mode, cell="bf16")
     if name == "stale_c":
-        return replace(mode, stale_c=(0, 1, 2, 3)) if layer == 0 else mode
+        return replace(mode, stale_c=tuple(range(min(4, width)))) if layer == 0 else mode
     if name == "swap_fo":
-        return replace(mode, swap_fo=(0,)) if layer == 1 else mode
+        return replace(mode, swap_fo=(0,)) if layer == min(1, n_layers - 1) else mode
     return mode
 
 
 def _teacher_forced(emb, layers, ids, states, modes, mutant=None):
     xs = [emb[ids]] + states[:-1]
-    stats = [D.ratio_stats(states[l], *D.teacher_forced_layer(xs[l], states[l], layers[l], _mutant(modes[l], l, mutant)))
-             for l in range(len(layers))]
+    n, width = len(layers), layers[0]["w_hh"].shape[1]
+    assert mutant is None or any(_mutant(modes[l], l, mutant, n, width) != modes[l] for l in range(n)), mutant
+    stats = [D.ratio_stats(states[l], *D.teacher_forced_layer(xs[l], states[l], layers[l],
+                                                            _mutant(modes[l], l, mutant, n, width)))
+             for l in range(n)]
     return max(s["max"] for s in stats), max(s["rms"] for s in stats)
 
 
@@ -52,19 +64,39 @@ def test_without_rounding_it_is_the_plain_lstm(small):
     assert float(bound.max()) == 0.0
 
 
-@pytest.mark.parametrize("flags,env", [(0, None), (0, {"IE_FAST_MATH": 0}), (0, {"IE_GX_BF16": 0}),
-                                       (0, {"IE_FUSE_LAST": 0}), (D.IE_CFG_FP32, None)])
-def test_free_running_emulation_inside_bound_and_mutants_outside(small, flags, env):
-    """Observed here (float32 emulation, torch gates): design max ratio 0.43 (default) to 0.98 (IEEE-like gates), every
-    mutant's max ratio >= 7.8 and its RMS ratio >= 1.7, i.e. at least 8x beyond the design."""
-    emb, layers, ids = small
+KNOB_SETS = [(0, None), (0, {"IE_FAST_MATH": 0}), (0, {"IE_GX_BF16": 0}), (0, {"IE_FUSE_LAST": 0}), (D.IE_CFG_FP32, None)]
+
+
+def _emulation_inside_bound_and_mutants_outside(emb, layers, ids, flags, env, tag=None):
     modes = D.layer_modes(len(layers), flags, env)
     states = D.free_run(emb, layers, ids, modes, torch.float32)
     mx, rms = _teacher_forced(emb, layers, ids, states, modes)
     assert mx <= 1.0 and rms <= 0.05, (mx, rms)
     for name in ("gx_bf16", "cell_bf16", "stale_c", "swap_fo"):
         m_mx, m_rms = _teacher_forced(emb, layers, ids, states, modes, name)
-        assert m_mx > 4.0 or m_rms > 1.0, (name, m_mx, m_rms)
+        if (tag, name, modes[0].gates) in WEAK:
+            assert m_mx > 1.0 and m_mx > 8 * mx, (name, m_mx, mx)
+        else:
+            assert m_mx > 4.0 or m_rms > 1.0, (name, m_mx, m_rms)
+
+
+@pytest.mark.parametrize("flags,env", KNOB_SETS)
+def test_free_running_emulation_inside_bound_and_mutants_outside(small, flags, env):
+    """Observed here (float32 emulation, torch gates): design max ratio 0.43 (default) to 0.98 (IEEE-like gates), every
+    mutant's max ratio >= 7.8 and its RMS ratio >= 1.7, i.e. at least 8x beyond the design."""
+    _emulation_inside_bound_and_mutants_outside(*small, flags, env)
+
+
+@pytest.mark.parametrize("tag", list(SHAPES))
+@pytest.mark.parametrize("flags,env", KNOB_SETS)
+def test_free_running_emulation_at_other_shape_classes(tag, flags, env):
+    """The same at one layer, emb > hid and width 1.  Observed: one layer and emb > hid, design max ratio 0.004-0.98,
+    every mutant's max >= 6.7 and RMS >= 1.3; width 1, see WEAK."""
+    shape = SHAPES[tag]
+    ref = R.make_encoder(7, shape[3], shape[1], shape[2], shape[0], scale=2.0)
+    emb, layers = ref.export_weights()
+    ids = np.stack(R.synthetic_ids(32, 33, seed=3, vocab_sz=shape[3]))
+    _emulation_inside_bound_and_mutants_outside(emb, layers, ids, flags, env, tag)
 
 
 def test_layer_modes_follow_the_knobs():
@@ -74,6 +106,11 @@ def test_layer_modes_follow_the_knobs():
     fp32 = D.layer_modes(3, D.IE_CFG_FP32, {"IE_GX_BF16": 1, "IE_FAST_MATH": 1})
     assert all(m.segs == 3 and m.gx == "f32" and m.gates == "ieee" for m in fp32)
     assert D.layer_modes(2, D.IE_CFG_ACCURATE_GATES)[0].gates == "exp"
+    # one layer: layer 0 reads the fp16 per-token table and is never fused (the fused layer needs a previous layer's ring)
+    assert [m.gx for m in D.layer_modes(1)] == ["fp16"]
+    assert [m.gx for m in D.layer_modes(1, 0, {"IE_GX_BF16": 0})] == ["f32"]
+    assert [(m.segs, m.gx) for m in D.layer_modes(1, D.IE_CFG_FP32)] == [(3, "f32")]
+    assert [m.gx for m in D.layer_modes(2)] == ["fp16", "fused"]
 
 
 def test_pool_restates_the_kernel_and_mutants_differ():

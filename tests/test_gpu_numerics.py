@@ -99,15 +99,17 @@ def test_gemm_table_shape_row_sample(out, segs):
 
 
 # ------------------------------------------------------------------------------------------------ b. recurrent kernel
-def _mutate(mode, layer, name):
+def _mutate(mode, layer, name, n_layers, width):
+    """Mutant `name` of layer `layer`'s arithmetic: stale c on the first min(4, width) units of layer 0 (width = layer 0's
+    hidden units), f/o swapped for unit 0 of layer 1 (of layer 0 in a one-layer model)."""
     if name == "gx_bf16":
         return replace(mode, gx="bf16") if mode.gx in ("fp16", "f32") else mode
     if name == "cell_bf16":
         return replace(mode, cell="bf16")
     if name == "stale_c":
-        return replace(mode, stale_c=(0, 1, 2, 3)) if layer == 0 else mode
+        return replace(mode, stale_c=tuple(range(min(4, width)))) if layer == 0 else mode
     if name == "swap_fo":
-        return replace(mode, swap_fo=(0,)) if layer == 1 else mode
+        return replace(mode, swap_fo=(0,)) if layer == min(1, n_layers - 1) else mode
     return mode
 
 
@@ -125,12 +127,16 @@ def _rows(B, extra=4, seed=0):
 
 def _teacher_forced_stats(enc, emb, layers, ids, modes, rows):
     """max / RMS of |dh| / bound over every layer, step and unit of `rows`, for the design and for every mutant."""
-    states = [torch.from_numpy(enc._debug_layer_states(l, ids)[rows]).to(_cuda()) for l in range(len(layers))]
+    n_layers, width = len(layers), np.asarray(layers[0]["w_hh"]).shape[1]
+    for name in MUTANTS:   # a mutant that changes no layer's arithmetic would pass as a negative control of nothing
+        assert any(_mutate(modes[l], l, name, n_layers, width) != modes[l] for l in range(n_layers)), name
+    states = [torch.from_numpy(enc._debug_layer_states(l, ids)[rows]).to(_cuda()) for l in range(n_layers)]
     xs = [torch.from_numpy(emb[ids[rows]]).to(_cuda())] + states[:-1]
     out = {}
     for name in (None,) + MUTANTS:
-        st = [D.ratio_stats(states[l], *D.teacher_forced_layer(xs[l], states[l], layers[l], _mutate(modes[l], l, name)))
-              for l in range(len(layers))]
+        st = [D.ratio_stats(states[l], *D.teacher_forced_layer(xs[l], states[l], layers[l],
+                                                              _mutate(modes[l], l, name, n_layers, width)))
+              for l in range(n_layers)]
         out[name or "design"] = (max(s["max"] for s in st), max(s["rms"] for s in st))
     return out
 

@@ -52,6 +52,9 @@ PROTOTYPES = {
                                 C.c_void_p, C.c_int32]),
     "ie_debug_gemm_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_int32, C.c_void_p, C.c_int32]),
+    "ie_debug_gemm_frag": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                     C.c_int32, C.c_void_p, C.c_int32]),
+    "ie_debug_epilogue_layout": (C.c_int64, [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "ie_debug_layer_states": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                         C.c_void_p]),
 }

@@ -191,15 +191,18 @@ int plan_layers(ie_encoder* h) {
   return IE_OK;
 }
 
-// torch gate-major rows [4*out] -> the recurrent kernel's column order; -1 marks zero padding rows.  Units go in groups
-// of four = 16 columns; unit q of a group has (i, f) at columns 2q, 2q+1 and (g, o) at 8+2q, 9+2q -- exactly the
-// columns one thread holds in a wgmma accumulator fragment (lstm_layer.cu), so a thread owns all four gates of a unit.
+// torch gate-major rows [4*out] -> the recurrent kernel's column order; -1 marks zero padding rows.  A 256-column tile
+// holds 64 units in 16 chunks of 16 columns; chunk m = 4s + e (s, e = 0..3) of the quad lane q has (i, f) at columns
+// 2q, 2q+1 and (g, o) at 8+2q, 9+2q of the chunk -- exactly the columns lane q holds in a wgmma accumulator fragment
+// (lstm_layer.cu), so a thread owns all four gates of a unit -- for unit 16s + 4q + e of the tile: a thread's units come
+// in runs of four (one 16-byte access of c, one 8-byte store of h) and a warp's access covers whole sectors of a row.
+// Only the N position of a weight row moves, so every accumulator element sums the same products in the same order.
 std::vector<int> slice_perm(const Layer& L) {
   std::vector<int> perm(4 * static_cast<size_t>(L.out_pad));
   for (int unit = 0; unit < L.out_pad; ++unit)
     for (int g = 0; g < 4; ++g) {
-      const int q = unit & 3;
-      const size_t col = static_cast<size_t>(unit >> 2) * 16 + (g < 2 ? 2 * q + g : 8 + 2 * q + (g - 2));
+      const int u = unit & 63, s = u >> 4, q = (u >> 2) & 3, e = u & 3;
+      const size_t col = static_cast<size_t>(unit >> 6) * 256 + (4 * s + e) * 16 + (g < 2 ? 2 * q + g : 8 + 2 * q + (g - 2));
       perm[col] = unit < L.out ? g * L.out + unit : -1;
     }
   return perm;
@@ -301,6 +304,7 @@ void fill_gemm(const ie_encoder* h, const Layer& L, ie::GemmArgs& g) {
   g.bn = L.bn;
   g.act = 0;
   g.out_bf16 = h->gx_bf16 ? 2 : 0;  // fp16 or f32
+  g.frag = 1;                        // Gx / table rows in the recurrent kernel's fragment order, bias likewise
   g.num_sms = h->num_sms;
   g.segs = h->segs;
   g.abort_flag = h->err.as<unsigned>() + 1;
@@ -685,8 +689,11 @@ int ie_encoder_load_layer(ie_encoder* h, int32_t layer, const float* w_ih, const
   if (rc != IE_OK) return rc;
   rc = upload_sliced(w_hh, 4 * L.out, L.out, perm, L.kh_pad, h->segs, L.w_hh, h->own_stream);
   if (rc != IE_OK) return rc;
+  // b_ih + b_hh in the fragment order of the Gx it is folded into (kernels.h frag_index, f32): the projection GEMM and
+  // the fused last layer read it as one float4 (i, f, g, o) per unit
   std::vector<float> bias(perm.size());
-  for (size_t r = 0; r < perm.size(); ++r) bias[r] = perm[r] < 0 ? 0.0f : b_ih[perm[r]] + b_hh[perm[r]];
+  for (size_t r = 0; r < perm.size(); ++r)
+    bias[r / 256 * 256 + ie::frag_index(static_cast<int>(r % 256), 4)] = perm[r] < 0 ? 0.0f : b_ih[perm[r]] + b_hh[perm[r]];
   CK(L.bias.reserve(bias.size() * sizeof(float)));
   CK(cudaMemcpy(L.bias.p, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
   if (layer == h->cfg.n_layers - 1 && layer > 0 && h->segs == 1) {
@@ -997,11 +1004,14 @@ void ie_mlp_destroy(ie_mlp* m) {
   delete m;
 }
 
-int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
-                     int32_t out_type, int32_t segs, float* d, int32_t device) {
+// frag: store in the fragment order of the encoder's input projections (kernels.h frag_index), undone here on the host
+static int debug_gemm(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
+                      int32_t out_type, int32_t segs, float* d, int32_t device, bool frag) {
   if (a == nullptr || b == nullptr || d == nullptr || M < 1 || N < 1 || K < 1) return fail(IE_ERR_INVALID, "bad argument");
   if (act < 0 || act > 2 || out_type < 0 || out_type > 2 || (out_type == 2 && act != 0) || (segs != 1 && segs != 3))
     return fail(IE_ERR_INVALID, "act=%d out_type=%d segs=%d not supported", act, out_type, segs);
+  if (frag && (bias == nullptr || act != 0 || out_type == 1 || N % 256 != 0))
+    return fail(IE_ERR_INVALID, "fragment order needs a bias, act 0, f32 or fp16 output and N %% 256 == 0");
   CK(cudaSetDevice(device));
   int sms = 132;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
@@ -1011,6 +1021,7 @@ int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t 
   if (n16 >= 240 && n16 % 240 == 0) bn = 240;
   else if (n16 >= 128) bn = 128;
   else bn = n16;
+  if (frag) bn = 256;
   const int n_pad = static_cast<int>(round_up(N, bn));
   // split-bf16 operands are [hi(k_pad) | lo(k_pad)] per row, as upload_sliced lays out the encoder's weights
   const int ld = segs == 3 ? 2 * k_pad : k_pad;
@@ -1029,7 +1040,11 @@ int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t 
   CK(ie::launch_convert_rows(fb.as<float>(), K, K, nullptr, N, bb.as<__nv_bfloat16>(), ld, lo_off, s));
   if (bias) {
     std::vector<float> bp(n_pad, 0.0f);
-    std::copy(bias, bias + N, bp.begin());
+    if (frag) {
+      for (int n = 0; n < N; ++n) bp[n / 256 * 256 + ie::frag_index(n % 256, 4)] = bias[n];
+    } else {
+      std::copy(bias, bias + N, bp.begin());
+    }
     CK(db.reserve(n_pad * 4));
     CK(cudaMemcpy(db.p, bp.data(), n_pad * 4, cudaMemcpyHostToDevice));
   }
@@ -1040,8 +1055,24 @@ int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t 
   g.bias = bias ? db.as<float>() : nullptr;
   g.m_pad = m_pad; g.n_pad = n_pad; g.k_pad = k_pad;
   g.m_store = M; g.n_store = n_pad; g.bn = bn; g.act = act; g.out_bf16 = out_type; g.num_sms = sms; g.segs = segs;
+  g.frag = frag ? 1 : 0;
   CK(ie::launch_gemm_bf16(g, s));
-  if (out_type == 0) {
+  if (frag) {
+    // raw rows, then column n of each row from position frag_index(n % 256) of its tile
+    std::vector<uint8_t> raw(static_cast<size_t>(M) * n_pad * elt);
+    CK(cudaMemcpy(raw.data(), dd.p, raw.size(), cudaMemcpyDeviceToHost));
+    for (size_t r = 0; r < static_cast<size_t>(M); ++r)
+      for (int n = 0; n < N; ++n) {
+        const size_t src = r * n_pad + n / 256 * 256 + ie::frag_index(n % 256, static_cast<int>(elt));
+        if (out_type == 0) {
+          std::memcpy(d + r * N + n, raw.data() + src * 4, 4);
+        } else {
+          __half_raw h;
+          std::memcpy(&h.x, raw.data() + src * 2, 2);
+          d[r * N + n] = __half2float(__half(h));
+        }
+      }
+  } else if (out_type == 0) {
     CK(cudaMemcpy2D(d, static_cast<size_t>(N) * 4, dd.p, static_cast<size_t>(n_pad) * 4, static_cast<size_t>(N) * 4, M,
                     cudaMemcpyDeviceToHost));
   } else {
@@ -1061,6 +1092,30 @@ int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t 
     }
   }
   return IE_OK;
+}
+
+int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
+                     int32_t out_type, int32_t segs, float* d, int32_t device) {
+  return debug_gemm(a, b, bias, M, N, K, act, out_type, segs, d, device, false);
+}
+
+int ie_debug_gemm_frag(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t out_type,
+                       int32_t segs, float* d, int32_t device) {
+  return debug_gemm(a, b, bias, M, N, K, 0, out_type, segs, d, device, true);
+}
+
+int64_t ie_debug_epilogue_layout(int32_t out_units, int32_t* perm, int64_t cap, int32_t* frag2, int32_t* frag4) {
+  if (out_units < 1) return fail(IE_ERR_INVALID, "out_units=%d must be >= 1", out_units);
+  Layer L;
+  L.out = out_units;
+  L.out_pad = static_cast<int>(round_up(out_units, 64));
+  const std::vector<int> p = slice_perm(L);
+  if (perm != nullptr && cap >= static_cast<int64_t>(p.size())) std::copy(p.begin(), p.end(), perm);
+  for (int c = 0; c < 256; ++c) {
+    if (frag2 != nullptr) frag2[c] = ie::frag_index(c, 2);
+    if (frag4 != nullptr) frag4[c] = ie::frag_index(c, 4);
+  }
+  return static_cast<int64_t>(p.size());
 }
 
 int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,

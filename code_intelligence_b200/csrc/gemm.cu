@@ -37,7 +37,7 @@ constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
 constexpr uint32_t kBBytes = kBlockN * kBlockK * 2;
 constexpr uint32_t kGemmStageBytes = kABytes + kBBytes;
 
-template <typename OutT, int ACT>
+template <typename OutT, int ACT, bool FRAG>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, OutT* __restrict__ D,
                  const float* __restrict__ bias, int m_store, int n_store, long long ldd, int num_m_blocks,
@@ -140,6 +140,44 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wgmma_wait<0>();
       wgmma_fence_regs(d);
       if (signal && prev >= 0) mbar_arrive(&empty_bar[prev]);
+      if constexpr (FRAG) {
+        // fragment order (kernels.h frag_index): this thread's values of a row are one run of 64 (m-major, gates
+        // i, f, g, o), stored as 16-byte chunks at position 4k + q of the row's tile; the bias is in the same order, as
+        // f32 (one float4 per m), loaded once for both rows
+        constexpr int kPer = 16 / static_cast<int>(sizeof(OutT));   // values per chunk: 8 fp16 or 4 f32
+        const float4* bq = reinterpret_cast<const float4*>(bias) + n_blk * (kBlockN / 4) + q;
+        OutT* drow[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr)
+          drow[hr] = D + static_cast<long long>(m_blk * kBlockM + rbase + 8 * hr) * ldd + n_blk * kBlockN + q * kPer;
+#pragma unroll
+        for (int k = 0; k < 64 / kPer; ++k) {
+          float4 b[kPer / 4];
+#pragma unroll
+          for (int i = 0; i < kPer / 4; ++i) b[i] = __ldg(bq + 4 * (k * (kPer / 4) + i));
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            if (m_blk * kBlockM + rbase + 8 * hr >= m_store) continue;
+            float x[kPer];
+#pragma unroll
+            for (int i = 0; i < kPer / 4; ++i) {
+              const int m = k * (kPer / 4) + i;
+              x[4 * i + 0] = d[8 * m + 2 * hr] + b[i].x;
+              x[4 * i + 1] = d[8 * m + 2 * hr + 1] + b[i].y;
+              x[4 * i + 2] = d[8 * m + 4 + 2 * hr] + b[i].z;
+              x[4 * i + 3] = d[8 * m + 4 + 2 * hr + 1] + b[i].w;
+            }
+            uint4 v;
+            if constexpr (sizeof(OutT) == 4) {
+              v = make_uint4(__float_as_uint(x[0]), __float_as_uint(x[1]), __float_as_uint(x[2]), __float_as_uint(x[3]));
+            } else {
+              v = make_uint4(pack_f16x2(x[0], x[1]), pack_f16x2(x[2], x[3]), pack_f16x2(x[4], x[5]), pack_f16x2(x[6], x[7]));
+            }
+            *reinterpret_cast<uint4*>(drow[hr] + 4 * k * kPer) = v;
+          }
+        }
+        continue;
+      }
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int row = m_blk * kBlockM + rbase + 8 * hr;
@@ -207,9 +245,9 @@ cudaError_t launch_gemm_bf16(const GemmArgs& g, cudaStream_t stream) {
   // (4 MB at K = 1024) and ~grid/16 B tiles, far inside the 50 MB L2 next to the output stream
   const int panel = 16;
 
-#define IE_LAUNCH(OUT, ACT)                                                                                        \
+#define IE_LAUNCH(OUT, ACT, FRAG)                                                                                  \
   do {                                                                                                             \
-    auto kfn = gemm_bf16_kernel<OUT, ACT>;                                                                         \
+    auto kfn = gemm_bf16_kernel<OUT, ACT, FRAG>;                                                                       \
     e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));            \
     if (e != cudaSuccess) return e;                                                                                \
     kfn<<<grid, kGemmThreads, smem, stream>>>(tmA, tmB, reinterpret_cast<OUT*>(g.d), g.bias, g.m_store, g.n_store, \
@@ -217,17 +255,24 @@ cudaError_t launch_gemm_bf16(const GemmArgs& g, cudaStream_t stream) {
                                               g.k_pad, g.abort_flag, spin_limit, g.diag);                          \
   } while (0)
 
-  if (g.out_bf16 == 2) {
+  if (g.frag) {
+    // fragment order: whole 256-column tiles, a bias in the same order, 16-byte aligned rows
+    if (g.act != 0 || g.out_bf16 == 1 || g.bias == nullptr || g.n_store % kBlockN || g.n_store != g.n_pad ||
+        (g.ldd * (g.out_bf16 == 2 ? 2 : 4)) % 16)
+      return cudaErrorInvalidValue;
+    if (g.out_bf16 == 2) IE_LAUNCH(__half, 0, true);
+    else IE_LAUNCH(float, 0, true);
+  } else if (g.out_bf16 == 2) {
     if (g.act != 0) return cudaErrorInvalidValue;
-    IE_LAUNCH(__half, 0);
+    IE_LAUNCH(__half, 0, false);
   } else if (g.out_bf16) {
-    if (g.act == 0) IE_LAUNCH(__nv_bfloat16, 0);
-    else if (g.act == 1) IE_LAUNCH(__nv_bfloat16, 1);
-    else IE_LAUNCH(__nv_bfloat16, 2);
+    if (g.act == 0) IE_LAUNCH(__nv_bfloat16, 0, false);
+    else if (g.act == 1) IE_LAUNCH(__nv_bfloat16, 1, false);
+    else IE_LAUNCH(__nv_bfloat16, 2, false);
   } else {
-    if (g.act == 0) IE_LAUNCH(float, 0);
-    else if (g.act == 1) IE_LAUNCH(float, 1);
-    else IE_LAUNCH(float, 2);
+    if (g.act == 0) IE_LAUNCH(float, 0, false);
+    else if (g.act == 1) IE_LAUNCH(float, 1, false);
+    else IE_LAUNCH(float, 2, false);
   }
 #undef IE_LAUNCH
   return cudaGetLastError();

@@ -14,6 +14,20 @@ namespace ie {
 cudaError_t make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows, uint64_t ld,
                               uint32_t box_inner, uint32_t box_rows);
 
+// ---- fragment order of a 256-column tile (Gx, the per-token table, the encoder's bias) -----------------------------
+// In a wgmma m64n256 accumulator, lane q = lane % 4 of a warp holds, for each of its rows, the 64 columns 16m + 2q + {0,1}
+// and 16m + 8 + 2q + {0,1} (m = 0..15) -- for the recurrent kernel the gates (i, f, g, o) of 16 hidden units.  In fragment
+// order these 64 values are one contiguous run per q, in that order (m-major, then i, f, g, o), cut into 16-byte chunks
+// that are interleaved over q: chunk k of lane q sits at chunk position 4k + q of the row's tile.  A warp's 16-byte
+// access of chunk k then covers 64 contiguous bytes of each of its rows.  Returns the element position inside the tile
+// of natural column c (0..255) for elements of `elem_bytes` (2: fp16, 4: f32) bytes.
+__host__ __device__ inline int frag_index(int c, int elem_bytes) {
+  const int q = (c & 7) >> 1;                                     // owning lane of the quad
+  const int ix = 4 * (c >> 4) + 2 * ((c >> 3) & 1) + (c & 1);    // position in that lane's run of 64 values
+  const int per_chunk = 16 / elem_bytes;
+  return (ix / per_chunk * 4 + q) * per_chunk + ix % per_chunk;
+}
+
 // ---- GEMM (gemm.cu) ----------------------------------------------------------------------------
 struct GemmArgs {
   const __nv_bfloat16* a;  // [m_pad, lda]   (split-bf16: [hi(k_pad) | lo(k_pad)] per row)
@@ -31,6 +45,7 @@ struct GemmArgs {
   unsigned* abort_flag;  // optional global word raised when a wait exceeds spin_limit (ptx.cuh abort protocol)
   long long spin_limit;  // SM cycles; 0 = default
   long long* diag;       // optional [4]: {clock64, globaltimer ns} at the start and end of CTA 0
+  int frag;              // 1: store D (and read bias) in fragment order (frag_index; act 0, f32 or fp16, n_store % 256 == 0)
 };
 cudaError_t launch_gemm_bf16(const GemmArgs& g, cudaStream_t stream);
 
@@ -45,11 +60,11 @@ struct LstmLayerArgs {
   CUtensorMap tm_x;        // pre_nkb > 0: the PREVIOUS layer's ring (slot t+1 = this layer's x_t), box {64, 128}
   int pre_nkb;             // > 0: fuse the input projection into the K loop -- pre_nkb = kin_pad / 64 k-blocks of
                            // x_t W_ih^T precede the recurrent ones; tm_w then covers [W_ih | W_hh] (inner kin_pad + kh_pad),
-                           // gx is unused and `bias` (b_ih + b_hh, permuted like the weight rows) is added instead
+                           // gx is unused and `bias` (b_ih + b_hh, permuted like the weight rows, fragment order) is added instead
   const float* bias;
   int mc;                  // 1: clusters of two CTAs share every h tile by TMA multicast (needs an even number of tiles)
   int mc_ctas;             // CTAs that can be co-resident in clusters of two (lstm_layer_max_ctas() of a check_only query)
-  const void* gx;          // f16 or f32 [rows, 4*out_pad] (bias folded in): row t*b_pad + brow of the chunk, or token id
+  const void* gx;          // f16 or f32 [rows, 4*out_pad] (bias folded in, fragment order): row t*b_pad + brow of the chunk, or token id
   const int* tok;          // optional time-major token ids of the whole call (per-token input-projection table)
   float* c;                // [b_pad, out_pad] cell state
   __nv_bfloat16* y;        // ring (slot 0 = h before the chunk (zeros at t0 = 0); slot t+1 = h_t, t chunk-local)

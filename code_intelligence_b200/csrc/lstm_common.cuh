@@ -5,6 +5,7 @@
 // Issue_Embeddings/flask_app/inference.py:57,68 (gate rows i|f|g|o, c_t = f*c_{t-1} + i*g, h_t = o*tanh(c_t));
 // pooling: inference.py:239 ([mean | max | last] over the first len_i steps).
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include "ptx.cuh"
@@ -47,27 +48,34 @@ __device__ __forceinline__ void lstm_cell1(float zi, float zf, float zg, float z
 }
 
 // ---- masked concat-pool accumulators in global memory ------------------------------------------------------------
-// pool_sum : f32, sequential sum over t (one add per timestep, in timestep order): an L2 reduction (red.add.f32) --
-//            no load, no accumulator registers.  The (step, batch) counter protocol of the persistent kernel orders
-//            step t's reduction after step t-1's (gpu-scope fence before the counter increment), so it is the same
-//            sequential f32 sum a register accumulator would give: identical bits on every path.
+// Natural unit order [row, out_pad]; the epilogue handles four adjacent units of one row at a time (one 16-byte access).
+// pool_sum : f32, sequential sum over t (one add per timestep, in timestep order): an L2 reduction (red.add.v4.f32 =
+//            four independent f32 adds) -- no load, no accumulator registers.  The (step, batch) counter protocol of the
+//            persistent kernel orders step t's reduction after step t-1's (gpu-scope fence before the counter
+//            increment), so it is the same sequential f32 sum a register accumulator would give: identical bits on
+//            every path.
 // pool_max : f32 running max; it travels like the cell state (read from L2 after the (t-1, batch) counter was seen)
 // pool_last: f32, h at t == len-1
-__device__ __forceinline__ void red_add_f32(float* p, float v) {
-  asm volatile("red.relaxed.gpu.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+__device__ __forceinline__ void red_add_v4_f32(float* p, float4 v) {
+  asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
+               "f"(v.w)
+               : "memory");
 }
-// po: offset of the unit in the [row, out_pad] accumulator arrays; tg: global timestep; len: valid length of the row
-__device__ __forceinline__ void pool_accumulate1(float* pool_sum, float* pool_max, float* pool_last, long long po,
-                                                 float hn, int tg, int len) {
+// po: offset of the first of the four units in the [row, out_pad] accumulator arrays (a multiple of 4); tg: global
+// timestep; len: valid length of the row
+__device__ __forceinline__ void pool_accumulate4(float* pool_sum, float* pool_max, float* pool_last, long long po,
+                                                 float4 hn, int tg, int len) {
   if (tg >= len) return;
+  float4* mp = reinterpret_cast<float4*>(pool_max + po);
   if (tg == 0) {
-    __stcg(pool_sum + po, hn);
-    __stcg(pool_max + po, hn);
+    __stcg(reinterpret_cast<float4*>(pool_sum + po), hn);
+    __stcg(mp, hn);
   } else {
-    red_add_f32(pool_sum + po, hn);
-    __stcg(pool_max + po, fmaxf(__ldcg(pool_max + po), hn));
+    red_add_v4_f32(pool_sum + po, hn);
+    const float4 m = __ldcg(mp);
+    __stcg(mp, make_float4(fmaxf(m.x, hn.x), fmaxf(m.y, hn.y), fmaxf(m.z, hn.z), fmaxf(m.w, hn.w)));
   }
-  if (tg == len - 1) __stcg(pool_last + po, hn);
+  if (tg == len - 1) __stcg(reinterpret_cast<float4*>(pool_last + po), hn);
 }
 
 // order-preserving u32 encoding of f32 (used by pr_curve.cu to sort scores as integers)
@@ -86,12 +94,15 @@ __host__ __device__ __forceinline__ float dec_max(uint32_t e) {
 #endif
 }
 
-// h_t in the ring: bf16 (hi); with `lo_off` > 0 also the bf16 residual h - hi at column offset lo_off (the split-bf16
-// fp32-accurate mode: h ~ hi + lo to ~16 mantissa bits)
-__device__ __forceinline__ void store_h1(__nv_bfloat16* yp, float hn, long long lo_off) {
-  const __nv_bfloat16 hi = __float2bfloat16_rn(hn);
-  *yp = hi;
-  if (lo_off > 0) yp[lo_off] = __float2bfloat16_rn(hn - __bfloat162float(hi));
+// h_t of four adjacent units in the ring: bf16 (hi), one 8-byte store; with `lo_off` > 0 also the bf16 residual
+// h - hi at column offset lo_off (the split-bf16 fp32-accurate mode: h ~ hi + lo to ~16 mantissa bits)
+__device__ __forceinline__ void store_h4(__nv_bfloat16* yp, float4 hn, long long lo_off) {
+  // hi as f32 (exactly representable: re-rounding it in pack_bf16x2 is the identity)
+  const float x = __bfloat162float(__float2bfloat16_rn(hn.x)), y = __bfloat162float(__float2bfloat16_rn(hn.y));
+  const float z = __bfloat162float(__float2bfloat16_rn(hn.z)), w = __bfloat162float(__float2bfloat16_rn(hn.w));
+  *reinterpret_cast<uint2*>(yp) = make_uint2(pack_bf16x2(x, y), pack_bf16x2(z, w));
+  if (lo_off > 0)
+    *reinterpret_cast<uint2*>(yp + lo_off) = make_uint2(pack_bf16x2(hn.x - x, hn.y - y), pack_bf16x2(hn.z - z, hn.w - w));
 }
 
 }  // namespace ie

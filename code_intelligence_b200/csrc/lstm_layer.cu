@@ -8,8 +8,9 @@
 // Work decomposition ("rotating schedule"):
 //   * an ITEM is 128 batch rows x one column tile of 256 accumulator columns = 64 hidden units x (i,f,g,o).  Weight rows
 //     are pre-permuted (api.cu slice_perm) so that the wgmma fragment of a thread holds all four gates of a unit: inside
-//     each 16-column chunk, columns 2q, 2q+1 are (i, f) and 8+2q, 9+2q are (g, o) of the chunk's unit q -- the cell update
-//     needs no cross-thread traffic;
+//     16-column chunk m = 4s + e, columns 2q, 2q+1 are (i, f) and 8+2q, 9+2q are (g, o) of unit 16s + 4q + e -- the cell
+//     update needs no cross-thread traffic, and a thread's units come in runs of four (16-byte c, 8-byte h accesses);
+//     Gx is stored in the matching fragment order (kernels.h frag_index): 16-byte loads;
 //   * the items  n = t * C + g * 2 tiles + half * tiles + j  (C = ng * 2 tiles; timestep t, batch g, row half, column
 //     tile j) are dealt round-robin in that global order over the P resident CTAs: CTA p runs items p, p + P, ...  Item n
 //     needs h_{t-1} of batch g, i.e. items of step t-1 with smaller indices; every CTA walks its items in increasing
@@ -31,8 +32,6 @@
 // either gets the whole grid resident or fails; a wait that still exceeds its limit raises the abort protocol of ptx.cuh.
 #include <cmath>
 
-#include <type_traits>
-
 #include <cuda_fp16.h>
 
 #include "kernels.h"
@@ -50,10 +49,6 @@ constexpr int kLRows = 128;             // batch rows per item
 constexpr uint32_t kHBytes = kLRows * 64 * 2;
 constexpr uint32_t kWBytes = kLTileN * 64 * 2;
 constexpr uint32_t kStageBytes = kHBytes + kWBytes;
-// units of the epilogue whose loads are in flight together (divides 16).  Larger groups spill: the consumers already
-// hold 128 accumulators within the 168 registers a thread has at 384 threads per SM
-constexpr int kEpiGroup = 2;
-static_assert(16 % kEpiGroup == 0, "kEpiGroup must divide 16");
 
 __device__ __forceinline__ void st_release_cta(uint32_t* p, uint32_t v) {
   asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
@@ -76,9 +71,9 @@ __device__ __forceinline__ void wait_seq_ge(const uint32_t* p, uint32_t target, 
 }
 
 struct KArgs {
-  const void* gx;        // f16 or f32 [rows, 4*out_pad]; row = t_local*b_pad + brow, or the token id (TOK)
+  const void* gx;        // f16 or f32 [rows, 4*out_pad] in fragment order; row = t_local*b_pad + brow, or the token id (TOK)
   const int* tok;        // TOK: time-major token ids of the whole call, index (t0 + t)*b_pad + brow
-  const float* bias;     // FUSE: b_ih + b_hh in the permuted column order (takes the place of Gx)
+  const float* bias;     // FUSE: b_ih + b_hh, permuted, in fragment order (takes the place of Gx)
   float* cstate;         // [b_pad, out_pad]
   __nv_bfloat16* y;      // ring [(T+1)*b_pad, ldy] of this time chunk: slot 0 = h before the chunk, slot t+1 = h_t
   float* raw;            // optional [b_pad, T_total, raw_ld]
@@ -293,60 +288,63 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
         const int len = POOL ? a.lengths[brow] : 1;
         const long long grow = TOK ? static_cast<long long>(__ldg(a.tok + static_cast<long long>(tg) * b_pad + brow))
                                    : static_cast<long long>(t) * b_pad + brow;  // TOK: per-token projection table
-        const int unit0 = j * 64 + q;
+        const int unit0 = j * 64 + 4 * q;     // + 16 s: this thread's units of group s are unit0 + 16 s + 0..3
         float* cp = a.cstate + static_cast<long long>(brow) * a.out_pad + unit0;
         __nv_bfloat16* yrow = a.y + (static_cast<long long>(t + 1) * b_pad + brow) * a.ldy + unit0;
         const long long po = static_cast<long long>(brow) * a.out_pad + unit0;
-        const long long gbase = grow * (4ll * a.out_pad) + j * kLTileN + 2 * q;
-        // the 16 units run in groups of kEpiGroup: a group's loads (Gx or bias, c_{t-1}) are all issued before its
-        // stores, so their latencies overlap -- loads after the previous unit's stores would be a chain of 32
-        // dependent L2 / HBM round trips per item (the compiler cannot move a load above a store it may alias)
+        // this thread's run of 64 Gx values (or bias values) in the row's fragment-ordered tile: 16-byte chunk k at
+        // chunk position 4k + q (kernels.h frag_index)
+        const long long gtile = grow * (4ll * a.out_pad) + j * kLTileN;
+        // FUSE: the bias tile in the same order; the empty asm makes its address opaque per row, so that the compiler
+        // does not hoist the row-invariant bias loads out of the row loop (64 values held across it would spill)
+        const float* btile = FUSE ? a.bias + j * kLTileN : nullptr;
+        if constexpr (FUSE) asm volatile("" : "+l"(btile));
+        // the 16 units run in groups of four (one 16-byte c access, one 8-byte h store each): a group's loads (Gx or
+        // bias, c_{t-1}) are all issued before its stores, so their latencies overlap -- loads after the previous
+        // group's stores would be a chain of dependent L2 / HBM round trips per item (the compiler cannot move a load
+        // above a store it may alias)
 #pragma unroll
-        for (int m0 = 0; m0 < 16; m0 += kEpiGroup) {
-          // this thread's unit 4m+q of the tile: (i, f) at columns 16m + 2q (+1), (g, o) at 16m + 8 + 2q (+1)
-          using GxT = typename std::conditional<GXBF && !FUSE, __half2, float2>::type;
-          GxT gif[kEpiGroup], ggo[kEpiGroup];
-          float cprev[kEpiGroup];
+        for (int s = 0; s < 4; ++s) {
+          // accumulator chunk m = 4s + e holds unit 16s + 4q + e: (i, f) at d[8m + 2hr (+1)], (g, o) at d[8m + 4 + 2hr (+1)]
+          // Gx of the group's units e = 0..3, as loaded: fp16 -- two chunks of (i, f, g, o) x 2 units, issued here and
+          // widened only where they are added; f32 Gx and the bias (FUSE) -- one chunk of (i, f, g, o) per unit, loaded
+          // next to its use (four float4 in flight here would spill)
+          uint4 gh[2];
+          if constexpr (GXBF && !FUSE) {
+            const uint4* gp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(a.gx) + gtile) + q;
 #pragma unroll
-          for (int i = 0; i < kEpiGroup; ++i) {
-            const int m = m0 + i;
+            for (int i = 0; i < 2; ++i) gh[i] = __ldcs(gp + 4 * (2 * s + i));
+          }
+          const float4 cprev = (tg == 0) ? make_float4(0.0f, 0.0f, 0.0f, 0.0f)
+                                         : __ldcg(reinterpret_cast<const float4*>(cp + 16 * s));
+          const float cp4[4] = {cprev.x, cprev.y, cprev.z, cprev.w};
+          float cn[4], hn[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int m = 4 * s + e;
+            float4 gx;
             if constexpr (FUSE) {
-              gif[i] = __ldg(reinterpret_cast<const float2*>(a.bias + j * kLTileN + 2 * q + 16 * m));
-              ggo[i] = __ldg(reinterpret_cast<const float2*>(a.bias + j * kLTileN + 2 * q + 16 * m + 8));
+              gx = __ldg(reinterpret_cast<const float4*>(btile) + q + 4 * m);
             } else if constexpr (GXBF) {
-              const __half2* gp = reinterpret_cast<const __half2*>(reinterpret_cast<const __half*>(a.gx) + gbase + 16 * m);
-              gif[i] = __ldcs(gp);
-              ggo[i] = __ldcs(gp + 4);
+              const uint32_t w0 = (e & 1) ? gh[e >> 1].z : gh[e >> 1].x, w1 = (e & 1) ? gh[e >> 1].w : gh[e >> 1].y;
+              const float2 f01 = __half22float2(*reinterpret_cast<const __half2*>(&w0));
+              const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&w1));
+              gx = make_float4(f01.x, f01.y, f23.x, f23.y);
             } else {
-              const float2* gp = reinterpret_cast<const float2*>(reinterpret_cast<const float*>(a.gx) + gbase + 16 * m);
-              gif[i] = __ldcs(gp);
-              ggo[i] = __ldcs(gp + 4);
+              gx = __ldcs(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(a.gx) + gtile) + q + 4 * m);
             }
-            cprev[i] = (tg == 0) ? 0.0f : __ldcg(cp + 4 * m);
+            const float zi = d[8 * m + 2 * hr] + gx.x;
+            const float zf = d[8 * m + 2 * hr + 1] + gx.y;
+            const float zg = d[8 * m + 4 + 2 * hr] + gx.z;
+            const float zo = d[8 * m + 4 + 2 * hr + 1] + gx.w;
+            lstm_cell1(zi, zf, zg, zo, cp4[e], cn[e], hn[e], a.gate_mode);
           }
-#pragma unroll
-          for (int i = 0; i < kEpiGroup; ++i) {
-            const int m = m0 + i;
-            float2 gi, go;
-            if constexpr (GXBF && !FUSE) {
-              gi = __half22float2(gif[i]);
-              go = __half22float2(ggo[i]);
-            } else {
-              gi = gif[i];
-              go = ggo[i];
-            }
-            const float zi = d[8 * m + 2 * hr] + gi.x;
-            const float zf = d[8 * m + 2 * hr + 1] + gi.y;
-            const float zg = d[8 * m + 4 + 2 * hr] + go.x;
-            const float zo = d[8 * m + 4 + 2 * hr + 1] + go.y;
-            float cnew, hn;
-            lstm_cell1(zi, zf, zg, zo, cprev[i], cnew, hn, a.gate_mode);
-            __stcg(cp + 4 * m, cnew);
-            store_h1(yrow + 4 * m, hn, lo_off);
-            if (a.raw != nullptr)
-              a.raw[(static_cast<long long>(brow) * a.T_total + tg) * a.raw_ld + unit0 + 4 * m] = hn;
-            if constexpr (POOL) pool_accumulate1(a.pool_sum, a.pool_max, a.pool_last, po + 4 * m, hn, tg, len);
-          }
+          const float4 h4 = make_float4(hn[0], hn[1], hn[2], hn[3]);
+          __stcg(reinterpret_cast<float4*>(cp + 16 * s), make_float4(cn[0], cn[1], cn[2], cn[3]));
+          store_h4(yrow + 16 * s, h4, lo_off);
+          if (a.raw != nullptr)
+            *reinterpret_cast<float4*>(a.raw + (static_cast<long long>(brow) * a.T_total + tg) * a.raw_ld + unit0 + 16 * s) = h4;
+          if constexpr (POOL) pool_accumulate4(a.pool_sum, a.pool_max, a.pool_last, po + 16 * s, h4, tg, len);
         }
       }
       // publish (step t, batch g): h_t / c_t / pooling state visible

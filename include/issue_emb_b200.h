@@ -170,6 +170,19 @@ int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, 
 int ie_debug_gemm_ex(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K, int32_t act,
                      int32_t out_type, int32_t segs, float* d, int32_t device);
 
+/* Same GEMM (act 0, bias required, N a multiple of 256) with the store the encoder's input projections use: each
+ * 256-column tile of a row in fragment order (DESIGN.md section 3), the bias read in the same order.  The result is
+ * put back into natural column order on the host, so d [M,N] is comparable element for element with
+ * ie_debug_gemm_ex; out_type 0 = f32, 2 = fp16. */
+int ie_debug_gemm_frag(const float* a, const float* b, const float* bias, int32_t M, int32_t N, int32_t K,
+                       int32_t out_type, int32_t segs, float* d, int32_t device);
+
+/* Host-only test hook: the layout maps of the recurrent kernel for a layer of `out_units` hidden units.  Returns the
+ * number of weight rows 4*out_pad (out_pad = out_units rounded up to 64); if cap >= that, perm receives the torch
+ * gate-major row (g*out_units + unit) behind each of them, -1 for padding.  frag2 / frag4 [256] (each optional)
+ * receive the fragment-order position of each column of a 256-column tile for 2- and 4-byte elements. */
+int64_t ie_debug_epilogue_layout(int32_t out_units, int32_t* perm, int64_t cap, int32_t* frag2, int32_t* frag4);
+
 /* Debug / test hook: the hidden states of layer `layer` of an encode of ids [B, T] (zero initial state), as that
  * layer's recurrent kernel computed them: out [B, T, out_l] f32, out_l = n_hid, or emb_sz for the last layer.  The
  * hidden-state ring the next step and the next layer read holds their bf16 round-to-nearest-even (hi + lo in the

@@ -17,6 +17,7 @@ IE_OK, IE_ERR_INVALID, IE_ERR_CUDA, IE_ERR_OOM, IE_ERR_STATE, IE_ERR_TOKEN = 0, 
 IE_FLAG_DEVICE_PTRS = 1
 IE_MAX_BATCH = 3072          # upper bound; a handle's own limit is ie_encoder_max_batch() (1280 by default)
 IE_CFG_ACCURATE_GATES, IE_CFG_FP32, IE_CFG_F32_GX = 1, 2, 4
+IE_KNN_COSINE, IE_KNN_EUCLIDEAN = 0, 1
 
 
 class ie_config(C.Structure):
@@ -57,6 +58,13 @@ PROTOTYPES = {
     "ie_debug_epilogue_layout": (C.c_int64, [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "ie_debug_layer_states": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                         C.c_void_p]),
+    "ie_knn_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]),
+    "ie_knn_destroy": (None, [C.c_void_p]),
+    "ie_knn_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),
+    "ie_knn_search": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                C.c_void_p]),
+    "ie_knn_check_errors": (C.c_int, [C.c_void_p]),
+    "ie_debug_knn_shortlist": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

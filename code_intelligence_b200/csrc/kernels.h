@@ -120,4 +120,35 @@ constexpr int kPrMaxSamples = 16384;
 cudaError_t launch_pr_thresholds(const float* scores, const uint8_t* truth, int n, int n_labels, double p_thr,
                                  double r_thr, float* out_thr, double* out_prec, double* out_rec, cudaStream_t stream);
 
+// ---- exact k-nearest-neighbour search (knn.cu) ----------------------------------------------------------------------
+constexpr int kKnnCap = 512;          // candidate-buffer entries per (query, corpus slice): k' + a whole 256-row tile fit
+constexpr int kKnnMergeMax = 16384;   // S * k' bound: the merge sorts one query's candidates in shared memory
+constexpr int kKnnExtra = 32;         // k' = k + kKnnExtra rows are shortlisted by stage 1 and re-ranked exactly
+// f64 column mean of x [n, D] rounded to f32 -> center [k_pad] (zeros past D); partial: knn_center_workspace(D) bytes
+size_t knn_center_workspace(int D);
+cudaError_t launch_knn_center(const float* x, long long n, int D, int k_pad, double* partial, float* center,
+                              cudaStream_t stream);
+// rows [rows_pad] of src [rows, D] f32 -> dst [rows_pad, 2*k_pad] split-bf16 of x - center (zero rows past `rows`),
+// terms [rows_pad]: mode 0 (|x~|^2/2, 0), 1 (c.x~, 1/|x| or 0), 2 (q~.c + c2, 0); a non-finite value sets *err
+cudaError_t launch_knn_prep(const float* src, long long rows, long long rows_pad, int D, int k_pad, const float* center,
+                            double c2, int mode, __nv_bfloat16* dst, float2* terms, int* err, cudaStream_t stream);
+// corpus slices S and n-blocks per slice for nq queries against n rows
+void knn_plan(int nq, long long n, int kp, int num_sms, int* S, int* nbs);
+struct KnnStage1Args {
+  const __nv_bfloat16* qs;  // [m_pad, 2*k_pad] split-bf16 centred queries
+  const __nv_bfloat16* xs;  // [n, 2*k_pad] split-bf16 centred corpus
+  const float2* col;        // [round_up(n, 256)] corpus terms
+  const float2* rowt;       // [m_pad] query terms
+  uint2* cand;              // [nq][S][kKnnCap]
+  int* cnt;                 // [nq][S]
+  long long n;
+  int nq, m_pad, k_pad, S, nbs, kp, cosine, num_sms;
+};
+cudaError_t launch_knn_stage1(const KnnStage1Args& a, cudaStream_t stream);
+// per query row: best kp candidates; dbg_score != nullptr: write them ([rows, kp]) and stop; else exact distances
+// from Q [rows, D] and X [n, D] f32 and the best k -> out_dist / out_idx [rows, k]
+cudaError_t launch_knn_merge_rerank(const uint2* cand, const int* cnt, int rows, int S, int kp, const float* Q,
+                                    const float* X, int D, int cosine, int k, float* out_dist, int64_t* out_idx,
+                                    float* dbg_score, int64_t* dbg_idx, cudaStream_t stream);
+
 }  // namespace ie

@@ -191,6 +191,37 @@ int64_t ie_debug_epilogue_layout(int32_t out_units, int32_t* perm, int64_t cap, 
 int ie_debug_layer_states(ie_encoder* h, int32_t layer, const int64_t* ids, int32_t B, int32_t T, float* out,
                           int32_t flags, void* stream);
 
+/* Exact k-nearest-neighbour index over embeddings (similar-issue search).  Replaces the brute-force neighbour searches
+ * of the reference's notebooks: the FewShot notebook's oneshotlabeler (CosineSimilarity over every stored issue) and
+ * KNeighborsClassifier(metric='cosine'), and notebook 08's KNeighborsClassifier(weights='distance') label model.
+ *   Rows are numbered 0.. in insertion order.  ie_knn_search returns for each query the k stored rows nearest under
+ *   the metric, ascending by distance, ties to the lower index: dist [nq, k] f32 (sklearn kneighbors convention:
+ *   cosine 1 - cos, computed as |q/|q| - x/|x||^2 / 2; euclidean |q - x|; a zero vector has cosine distance 1 to
+ *   everything), idx [nq, k] int64.  The answer is float64 brute force on the f32 inputs whenever at most 32 rows
+ *   outside the exact top k score within 2 eps of the k-th (DESIGN.md section 2): a split-bf16 tensor-core pass over
+ *   the centred data shortlists k + 32 rows per query, which are re-ranked exactly.
+ *   Limits: 1 <= dim <= 8192, 1 <= k <= 64, k <= rows stored, nq >= 1, rows < 2^31 (IE_ERR_OOM when the device is
+ *   full).  Searching an empty index returns IE_ERR_STATE.
+ *   Host pointers: a NaN or infinite value returns IE_ERR_INVALID before anything is launched.  IE_FLAG_DEVICE_PTRS:
+ *   asynchronous on `stream`; non-finite input is reported by ie_knn_check_errors().  The first ie_knn_add fixes the
+ *   centre (the f32-rounded f64 mean of its rows) and waits for it. */
+#define IE_KNN_COSINE 0
+#define IE_KNN_EUCLIDEAN 1
+typedef struct ie_knn ie_knn;
+int ie_knn_create(int32_t dim, int32_t metric, int32_t device, ie_knn** out);
+void ie_knn_destroy(ie_knn* h);
+/* X [n, dim] f32, appended as rows size..size+n-1 */
+int ie_knn_add(ie_knn* h, const float* X, int64_t n, int32_t flags, void* stream);
+int ie_knn_search(ie_knn* h, const float* Q, int32_t nq, int32_t k, float* dist, int64_t* idx, int32_t flags,
+                  void* stream);
+/* IE_OK, or IE_ERR_INVALID if a non-finite value was seen in device-pointer input since the last check (waits for the
+ * last call on this handle; clears the state). */
+int ie_knn_check_errors(ie_knn* h);
+/* Debug / test hook, host pointers: stage 1 alone -- the k + 32 best rows of each query by the tensor-core score
+ * (larger is nearer; euclidean q~.x~ - |x~|^2/2, cosine q.x / |x|, with x~ = x - c), score descending, ties to the lower
+ * index: score [nq, k + 32] f32 and idx [nq, k + 32] int64 (-1 / -inf past the rows stored). */
+int ie_debug_knn_shortlist(ie_knn* h, const float* Q, int32_t nq, int32_t k, float* score, int64_t* idx);
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,7 @@ constexpr int kLRows = 128;             // batch rows per item
 constexpr uint32_t kHBytes = kLRows * 64 * 2;
 constexpr uint32_t kWBytes = kLTileN * 64 * 2;
 constexpr uint32_t kStageBytes = kHBytes + kWBytes;
+constexpr int kGxPrefetchAhead = 8;     // k-blocks before the end of an item's MMAs at which its Gx lines are prefetched
 
 __device__ __forceinline__ void st_release_cta(uint32_t* p, uint32_t v) {
   asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
@@ -252,6 +253,7 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
       decode(n, t, g, half, j);
       const int tg = a.t0 + t;  // global timestep
       int prev = -1;
+      const int kb_prefetch = max(pre + nkt - kGxPrefetchAhead, 0);
       for (int kb = 0; kb < pre + nkt; ++kb) {
         mbar_wait(&full[stage], phase, ab);
         if (kb == pre && signal && wg == 0) IE_TRACE(2, k);          // first h_{t-1} stage landed
@@ -262,6 +264,27 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) wgmma_m64n256k16(d, da + 2 * kk, db + 2 * kk, (kb | kk) != 0);
         wgmma_commit();
+        if constexpr (!FUSE && !TOK) {
+          // Gx rows of this item come from HBM (a layer's Gx is streamed once, far larger than L2): pull the lines this
+          // thread's epilogue will read into L2 a few k-blocks before the MMAs end, so that the epilogue's dependent
+          // load -> store groups wait on L2 instead of HBM round trips.  Not earlier: lines held in L2 through the
+          // whole MMA phase compete with the weight k-blocks.  Not for TOK: its row index is a token id that would
+          // have to be loaded first, and that load stalls the MMA issue (measured slower).  Lane q of a quad takes
+          // line q (fp16: 4 lines of 128 B per row tile; f32: 8).
+          if (kb == kb_prefetch) {
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              const int brow = g * 256 + half * kLRows + rbase + 8 * hr;
+              const long long gtile = (static_cast<long long>(t) * b_pad + brow) * (4ll * a.out_pad) + j * kLTileN;
+              if constexpr (GXBF) {
+                prefetch_l2(reinterpret_cast<const __half*>(a.gx) + gtile + 64 * q);
+              } else {
+                prefetch_l2(reinterpret_cast<const float*>(a.gx) + gtile + 32 * q);
+                prefetch_l2(reinterpret_cast<const float*>(a.gx) + gtile + 32 * q + 128);
+              }
+            }
+          }
+        }
         if (prev >= 0) {
           wgmma_wait<1>();
           if (signal) {

@@ -234,6 +234,10 @@ __device__ __forceinline__ void wait_flag_ge_relaxed(const unsigned* p, unsigned
 __device__ __forceinline__ void red_relaxed_add(unsigned* p, unsigned v) {
   asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
+// bring the 128-byte line holding `p` into L2 (no register result, no completion to wait for)
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

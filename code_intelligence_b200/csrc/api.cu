@@ -1175,11 +1175,20 @@ int knn_grow(DevBuf& b, size_t bytes, size_t keep, cudaStream_t s) {
   return IE_OK;
 }
 
-int knn_finite(const float* x, long long rows, int dim, const char* what) {
-  const long long cells = rows * dim;
-  for (long long i = 0; i < cells; ++i)
-    if (!std::isfinite(x[i]))
-      return fail(IE_ERR_INVALID, "%s[%lld][%lld] = %g is not finite", what, i / dim, i % dim, static_cast<double>(x[i]));
+// host input: every value finite, every row's norm 0 or in [kKnnNormMin, kKnnNormMax] (the prep kernel's check)
+int knn_check_rows(const float* x, long long rows, int dim, const char* what) {
+  for (long long r = 0; r < rows; ++r) {
+    const float* v = x + r * dim;
+    double s = 0.0;
+    for (int i = 0; i < dim; ++i) {
+      if (!std::isfinite(v[i]))
+        return fail(IE_ERR_INVALID, "%s[%lld][%d] = %g is not finite", what, r, i, static_cast<double>(v[i]));
+      s += static_cast<double>(v[i]) * v[i];
+    }
+    if (s > 0.0 && (s < ie::kKnnNormMin * ie::kKnnNormMin || s > ie::kKnnNormMax * ie::kKnnNormMax))
+      return fail(IE_ERR_INVALID, "%s row %lld has norm %g, outside the index's range [2^-48, 2^48] (0 is allowed)",
+                  what, r, std::sqrt(s));
+  }
   return IE_OK;
 }
 
@@ -1195,7 +1204,7 @@ int knn_search(ie_knn* h, const float* Q, int32_t nq, int32_t k, float* dist, in
   if (k > h->n) return fail(IE_ERR_INVALID, "k=%d exceeds the %lld rows of the index", k, h->n);
   const bool dev = (flags & IE_FLAG_DEVICE_PTRS) != 0 && dbg_score == nullptr;
   if (!dev) {
-    const int rc = knn_finite(Q, nq, h->dim, "Q");
+    const int rc = knn_check_rows(Q, nq, h->dim, "Q");
     if (rc != IE_OK) return rc;
   }
   cudaStream_t s;
@@ -1314,7 +1323,7 @@ int ie_knn_add(ie_knn* h, const float* X, int64_t n, int32_t flags, void* stream
   if (h->n + n >= (1ll << 31) - 256)
     return fail(IE_ERR_INVALID, "%lld + %lld rows exceed the index limit of 2^31", h->n, static_cast<long long>(n));
   if (!dev) {
-    const int rc = knn_finite(X, n, h->dim, "X");
+    const int rc = knn_check_rows(X, n, h->dim, "X");
     if (rc != IE_OK) return rc;
   }
   cudaStream_t s;
@@ -1371,7 +1380,9 @@ int ie_knn_check_errors(ie_knn* h) {
   if (w == 0) return IE_OK;
   CK(cudaMemset(h->err.p, 0, sizeof(w)));
   CK(cudaDeviceSynchronize());
-  return fail(IE_ERR_INVALID, "a non-finite value was seen in device input (an added row or a query)");
+  if (w & 1) return fail(IE_ERR_INVALID, "a non-finite value was seen in device input (an added row or a query)");
+  return fail(IE_ERR_INVALID, "a row of device input (an added row or a query) has a norm outside the index's range "
+                              "[2^-48, 2^48] (0 is allowed)");
 }
 
 }  // extern "C"

@@ -124,6 +124,10 @@ cudaError_t launch_pr_thresholds(const float* scores, const uint8_t* truth, int 
 constexpr int kKnnCap = 512;          // candidate-buffer entries per (query, corpus slice): k' + a whole 256-row tile fit
 constexpr int kKnnMergeMax = 16384;   // S * k' bound: the merge sorts one query's candidates in shared memory
 constexpr int kKnnExtra = 32;         // k' = k + kKnnExtra rows are shortlisted by stage 1 and re-ranked exactly
+// Every stored row and query has |x| = 0 or kKnnNormMin <= |x| <= kKnnNormMax (f64 norm of the f32 row): then every
+// stage-1 product, partial sum and score is finite and the split products stay clear of f32's subnormal range
+// (DESIGN.md section 2).  Host input outside it is refused; device input raises bit 2 of the error flag.
+constexpr double kKnnNormMin = 0x1p-48, kKnnNormMax = 0x1p48;
 // f64 column mean of x [n, D] rounded to f32 -> center [k_pad] (zeros past D); partial: knn_center_workspace(D) bytes
 size_t knn_center_workspace(int D);
 cudaError_t launch_knn_center(const float* x, long long n, int D, int k_pad, double* partial, float* center,

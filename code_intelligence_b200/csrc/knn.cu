@@ -19,9 +19,10 @@ namespace ie {
 
 namespace {
 
-// monotone map float -> uint32: larger score, larger key; every non-NaN score maps above 0 (0 = empty slot)
+// monotone map float -> uint32: larger score, larger key; every non-NaN score maps above 0 (0 = empty slot).  -0 is
+// keyed as +0, so an exact-zero score ties by index whichever sign the MMA or the epilogue gave it.
 __device__ __forceinline__ uint32_t order_key(float s) {
-  const uint32_t b = __float_as_uint(s);
+  const uint32_t b = __float_as_uint(s) == 0x80000000u ? 0u : __float_as_uint(s);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 __device__ __forceinline__ float key_score(uint32_t k) {
@@ -259,7 +260,7 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
 
 // One CTA per destination row r < rows_pad: x~ = x - c (f64) -> dst row [bf16(x~) | bf16(x~ - hi)] over k_pad columns
 // (zeros past D, and whole zero rows for r >= rows); terms[r] per `mode` (0 corpus euclidean, 1 corpus cosine,
-// 2 query); a non-finite input raises *err.
+// 2 query); a non-finite input raises bit 1 of *err, a row norm outside [kKnnNormMin, kKnnNormMax] (other than 0) bit 2.
 __global__ void knn_prep_rows_kernel(const float* __restrict__ src, long long rows, int D, int k_pad,
                                      const float* __restrict__ center, double c2, int mode, __nv_bfloat16* __restrict__ dst,
                                      float2* __restrict__ terms, int* err) {
@@ -291,6 +292,7 @@ __global__ void knn_prep_rows_kernel(const float* __restrict__ src, long long ro
   sc = block_sum(sc, red[2]);
   if (threadIdx.x == 0) {
     float2 t = make_float2(0.0f, 0.0f);
+    if (r < rows && sx2 > 0.0 && (sx2 < kKnnNormMin * kKnnNormMin || sx2 > kKnnNormMax * kKnnNormMax)) atomicOr(err, 2);
     if (r < rows) {
       if (mode == 0) t = make_float2(static_cast<float>(0.5 * st2), 0.0f);
       else if (mode == 1) t = make_float2(static_cast<float>(sc), sx2 > 0.0 ? static_cast<float>(1.0 / sqrt(sx2)) : 0.0f);

@@ -31,7 +31,11 @@ class IssueIndex:
     """Rows numbered 0.. in insertion order; ``search(Q, k)`` -> (dist (nq, k) float32, idx (nq, k) int64), ascending by
     distance, ties to the lower index.  Distances follow sklearn's ``kneighbors``: cosine 1 - cos (a zero vector is at
     distance 1 from everything), euclidean |q - x|.  ``X`` and ``Q`` are float32 numpy arrays (synchronous) or CUDA
-    float32 torch tensors (asynchronous on torch's current stream; results come back as CUDA tensors)."""
+    float32 torch tensors (asynchronous on torch's current stream; results come back as CUDA tensors).
+
+    Every row of ``X`` and ``Q`` must be finite with norm 0 or between 2^-48 and 2^48 (the range in which every
+    stage-1 score is finite, DESIGN.md section 2): numpy input outside it raises ValueError; CUDA input outside it makes
+    that call's answer undefined and is reported by ``check_errors``."""
 
     def __init__(self, dim: int, metric: str = "cosine", device: int = 0):
         if metric not in _METRICS:
@@ -91,8 +95,8 @@ class IssueIndex:
         return dist, idx
 
     def check_errors(self) -> None:
-        """Raise ValueError if a non-finite value reached the index through device-pointer input (waits for the last
-        call); host input is checked before anything is launched."""
+        """Raise ValueError if a non-finite value or a row outside the norm range reached the index through
+        device-pointer input (waits for the last call); host input is checked before anything is launched."""
         check(self._lib.ie_knn_check_errors(self._h))
 
     def _shortlist(self, Q, k: int):

@@ -200,11 +200,14 @@ int ie_debug_layer_states(ie_encoder* h, int32_t layer, const int64_t* ids, int3
  *   everything), idx [nq, k] int64.  The answer is float64 brute force on the f32 inputs whenever at most 32 rows
  *   outside the exact top k score within 2 eps of the k-th (DESIGN.md section 2): a split-bf16 tensor-core pass over
  *   the centred data shortlists k + 32 rows per query, which are re-ranked exactly.
+ *   With exact stage-1 scores (small-integer data, DESIGN.md section 2) ties resolve by index however many there are.
  *   Limits: 1 <= dim <= 8192, 1 <= k <= 64, k <= rows stored, nq >= 1, rows < 2^31 (IE_ERR_OOM when the device is
- *   full).  Searching an empty index returns IE_ERR_STATE.
- *   Host pointers: a NaN or infinite value returns IE_ERR_INVALID before anything is launched.  IE_FLAG_DEVICE_PTRS:
- *   asynchronous on `stream`; non-finite input is reported by ie_knn_check_errors().  The first ie_knn_add fixes the
- *   centre (the f32-rounded f64 mean of its rows) and waits for it. */
+ *   full).  Range: every added row and query has norm 0 or between 2^-48 and 2^48, which keeps every stage-1 score
+ *   finite.  Searching an empty index returns IE_ERR_STATE.
+ *   Host pointers: a NaN or infinite value, or a row outside the range, returns IE_ERR_INVALID before anything is
+ *   launched.  IE_FLAG_DEVICE_PTRS: asynchronous on `stream`; such input is reported by ie_knn_check_errors() (the
+ *   answers of the calls that saw it are undefined).  The first ie_knn_add fixes the centre (the f32-rounded f64 mean
+ *   of its rows) and waits for it. */
 #define IE_KNN_COSINE 0
 #define IE_KNN_EUCLIDEAN 1
 typedef struct ie_knn ie_knn;
@@ -214,8 +217,8 @@ void ie_knn_destroy(ie_knn* h);
 int ie_knn_add(ie_knn* h, const float* X, int64_t n, int32_t flags, void* stream);
 int ie_knn_search(ie_knn* h, const float* Q, int32_t nq, int32_t k, float* dist, int64_t* idx, int32_t flags,
                   void* stream);
-/* IE_OK, or IE_ERR_INVALID if a non-finite value was seen in device-pointer input since the last check (waits for the
- * last call on this handle; clears the state). */
+/* IE_OK, or IE_ERR_INVALID if a non-finite value or a row outside the range was seen in device-pointer input since the
+ * last check (waits for the last call on this handle; clears the state). */
 int ie_knn_check_errors(ie_knn* h);
 /* Debug / test hook, host pointers: stage 1 alone -- the k + 32 best rows of each query by the tensor-core score
  * (larger is nearer; euclidean q~.x~ - |x~|^2/2, cosine q.x / |x|, with x~ = x - c), score descending, ties to the lower

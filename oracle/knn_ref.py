@@ -111,6 +111,98 @@ def exactness_holds(s_row, eps_row, k, extra=32):
     return int((s_row[rest] >= sk - eps_row[rest] - e_top).sum()) <= extra
 
 
+# ---- lattice data: the whole device computation is exact, so the device can be checked bit for bit ----------------
+# Entries are small integers (|x_i| <= 3, D <= 8192 with |x_i| <= 1): bf16 holds them exactly (lo = 0), every dot
+# product and |x|^2 / 2 is an integer below 2^24, exact in f32 in any summation order.  The first add is a block and
+# its negation, so the f64 mean (the centre) is exactly 0, and so are a_q and b_x.  Cosine rows are +-1 on a
+# power-of-4 count of coordinates, so |x| is a power of two: r_x = 1/|x| is exact, and so are q/|q| - x/|x| and the f64
+# re-rank sum in any order.  Exact stage-1 scores mean that exact ties are real ties, which stage 1 must break by index.
+
+def lattice_rows(rng, n, D, metric, lo=-3, hi=3, nnz=None):
+    """(n, D) float32 lattice rows: euclidean entries uniform in [lo, hi]; cosine +-1 on `nnz` (a power of 4 <= D,
+    default the largest) random coordinates."""
+    if metric == "euclidean":
+        return rng.integers(lo, hi + 1, (n, D)).astype(np.float32)
+    if nnz is None:
+        nnz = 4 ** int(np.floor(np.log(D) / np.log(4)))
+    assert nnz <= D and 4 ** round(np.log(nnz) / np.log(4)) == nnz, nnz
+    X = np.zeros((n, D), np.float32)
+    cols = np.argsort(rng.random((n, D)), axis=1)[:, :nnz]
+    np.put_along_axis(X, cols, rng.choice(np.float32([-1, 1]), (n, nnz)), axis=1)
+    return X
+
+
+def with_zero_centre(B):
+    """The first add of a lattice index: B and -B, whose f64 mean is exactly 0."""
+    return np.vstack([B, -B])
+
+
+def lattice_scores(X, Q, metric, dot=None):
+    """Stage-1 scores (nq, n) float64 exactly as the device forms them on lattice data with centre 0: euclidean
+    acc - f32(|x|^2 / 2), cosine f32(acc * f32(1 / sqrt(|x|^2))) with the square root in f64 and r = 0 for a zero row,
+    acc = q.x (exact).  `dot` may pass a precomputed exact Q @ X.T.  Zeros are +0 (the device keys -0 as +0)."""
+    X = np.asarray(X, dtype=np.float64)
+    acc = np.asarray(Q, dtype=np.float64) @ X.T if dot is None else np.asarray(dot, dtype=np.float64)
+    x2 = (X * X).sum(1)
+    if metric == "euclidean":
+        s = acc - (0.5 * x2)[None, :]
+    else:
+        with np.errstate(divide="ignore"):
+            r = np.where(x2 > 0, 1.0 / np.sqrt(x2), 0.0).astype(np.float32)
+        s = (acc.astype(np.float32) * r[None, :]).astype(np.float64)
+    return s + 0.0
+
+
+def topk_exact(s, kp):
+    """The best kp of each row of scores s (nq, n) by (score descending, index ascending) -> (score (nq, kp) float32,
+    idx (nq, kp) int64), -inf / -1 past n (the device shortlist's convention)."""
+    nq, n = s.shape
+    order = np.lexsort((np.broadcast_to(np.arange(n), s.shape), -s), axis=1)[:, :kp]
+    score = np.full((nq, kp), -np.inf, np.float32)
+    idx = np.full((nq, kp), -1, np.int64)
+    m = min(n, kp)
+    score[:, :m] = np.take_along_axis(s, order, 1)[:, :m]
+    idx[:, :m] = order[:, :m]
+    return score, idx
+
+
+def lattice_distances(X, Q, metric, dot=None):
+    """Exact f64 distances (nq, n) on lattice data (sklearn convention, as `brute`): every value is the correctly
+    rounded f64 of the exact distance, so equal distances are exact ties."""
+    X = np.asarray(X, dtype=np.float64)
+    Q = np.asarray(Q, dtype=np.float64)
+    acc = Q @ X.T if dot is None else np.asarray(dot, dtype=np.float64)
+    x2 = (X * X).sum(1)[None, :]
+    q2 = (Q * Q).sum(1)[:, None]
+    if metric == "euclidean":
+        return np.sqrt(q2 - 2.0 * acc + x2)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        d = 1.0 - acc / (np.sqrt(q2) * np.sqrt(x2))   # |q|, |x| powers of two: exact
+    return np.where((q2 == 0) | (x2 == 0), 1.0, d)
+
+
+def lattice_brute(X, Q, k, metric, dot=None):
+    """Exact k nearest on lattice data, ties to the lower index -> (dist (nq, k) float32, idx (nq, k) int64)."""
+    d = lattice_distances(X, Q, metric, dot)
+    idx = np.lexsort((np.broadcast_to(np.arange(d.shape[1]), d.shape), d), axis=1)[:, :k]
+    return np.take_along_axis(d, idx, 1).astype(np.float32), idx
+
+
+def plan(nq, n, kp, num_sms, merge_max=16384):
+    """Restates ``knn_plan`` in csrc/knn.cu for one pass of nq <= 128 * num_sms queries: (S slices, nbs 256-row
+    blocks per slice) -- one wave of (128-row query block, slice) items, at most merge_max / kp slices -- and the merge's
+    sort size P (the power of two >= S * kp)."""
+    m_blocks = -(-nq // 128)
+    n_blocks = -(-n // 256)
+    s = min(max(1, num_sms // m_blocks), n_blocks, merge_max // kp)
+    nbs = -(-n_blocks // s)
+    S = -(-n_blocks // nbs)
+    P = 1
+    while P < S * kp:
+        P *= 2
+    return S, nbs, P
+
+
 def vote(neigh_ind, dist, Y, weights):
     """sklearn KNeighborsClassifier.predict_proba per 0/1 label, column of class 1, stacked -> (n, L)."""
     dist = np.asarray(dist, dtype=np.float64)

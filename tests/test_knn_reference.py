@@ -70,6 +70,55 @@ def test_vote_matches_sklearn_predict_proba(cfg):
     assert np.abs(vote_proba(i, d, Y, cfg.get("weights", "uniform")) - want).max() <= 1e-6
 
 
+@pytest.mark.parametrize("metric", ["cosine", "euclidean"])
+def test_lattice_scores_are_the_exact_stage1_scores(metric):
+    """On lattice data with the zero centre, the device-form restatement equals the exact f64 stage-1 score."""
+    rng = np.random.default_rng(11)
+    B = K.lattice_rows(rng, 40, 64, metric)
+    X = np.vstack([K.with_zero_centre(B), K.lattice_rows(rng, 300, 64, metric), np.zeros((2, 64), np.float32)])
+    Q = np.vstack([K.lattice_rows(rng, 30, 64, metric), -np.abs(X[:1]), np.zeros((1, 64), np.float32)])
+    c = K.center(X[:80])
+    assert (c == 0).all()
+    s = K.lattice_scores(X, Q, metric)
+    s1, _ = K.stage1_scores(X, Q, c, metric)
+    assert (s == s1).all()
+    assert (s.astype(np.float32).astype(np.float64) == s).all()   # every score is an f32 value
+    assert not np.signbit(s[s == 0]).any()
+    if metric == "cosine":   # |x| powers of two: the distances are 1 - s / |q|, exactly
+        d = K.lattice_distances(X, Q[:30], metric)
+        assert (d == 1.0 - s[:30] / np.sqrt((Q[:30].astype(np.float64) ** 2).sum(1))[:, None]).all()
+
+
+def test_topk_exact_equals_a_naive_sort():
+    rng = np.random.default_rng(12)
+    s = rng.integers(-4, 4, (20, 500)).astype(np.float64)   # hundreds of ties per score
+    s[3] = 0.0
+    for kp in (1, 33, 96, 500, 600):
+        score, idx = K.topk_exact(s, kp)
+        for r in range(s.shape[0]):
+            naive = sorted(range(s.shape[1]), key=lambda j: (-s[r, j], j))[:kp]
+            m = len(naive)
+            assert list(idx[r, :m]) == naive and (score[r, :m] == s[r, naive]).all()
+            assert (idx[r, m:] == -1).all() and (score[r, m:] == -np.inf).all()
+    d, i = K.lattice_brute(K.lattice_rows(rng, 700, 16, "euclidean", -1, 1), np.zeros((2, 16), np.float32), 64,
+                           "euclidean")
+    assert (np.diff(d, axis=1) >= 0).all()
+    for r in range(2):   # within one distance, ascending index
+        same = d[r, 1:] == d[r, :-1]
+        assert (i[r, 1:][same] > i[r, :-1][same]).all()
+
+
+def test_plan_restates_knn_plan():
+    # one query block: one slice per SM (capped by the merge), P = 16384 once S * k' > 8192
+    assert K.plan(128, 256 * 132 * 2, 96, 132) == (132, 2, 16384)
+    assert K.plan(128, 256 * 114 * 2, 96, 114) == (114, 2, 16384)
+    assert K.plan(100, 100_000, 37, 132) == (131, 3, 8192)
+    # many query blocks share the SMs; at least one slice; never more slices than blocks
+    assert K.plan(3000, 100_000, 42, 132) == (5, 79, 256)
+    assert K.plan(128 * 132, 1000, 33, 132) == (1, 4, 64)
+    assert K.plan(1, 300, 96, 132) == (2, 1, 256)
+
+
 def _bf16(x):
     """Round float32 to bf16 (nearest even), returned as float64."""
     u = np.asarray(x, dtype=np.float32).view(np.uint32).astype(np.uint64)

@@ -32,17 +32,20 @@ __device__ __forceinline__ float tanh_ieee(float x) {
 }
 
 // One hidden unit of one batch row.  z* = the accumulator (h_{t-1} W_hh^T, plus x_t W_ih^T when the input projection
-// rides the K loop) + Gx (x_t W_ih^T + b_ih + b_hh) or the bias; gate order i, f, g, o as in torch.
-__device__ __forceinline__ void lstm_cell1(float zi, float zf, float zg, float zo, float cprev, float& cnew, float& hn,
-                                           int gate_mode) {
-  if (gate_mode == kGatesFast) {
+// rides the K loop) + Gx (x_t W_ih^T + b_ih + b_hh) or the bias; gate order i, f, g, o as in torch.  The gate mode is a
+// template parameter so that an epilogue holds only the one gate path it runs.
+template <int GM>
+__device__ __forceinline__ void lstm_cell1(float zi, float zf, float zg, float zo, float cprev, float& cnew, float& hn) {
+  if constexpr (GM == kGatesFast) {
     cnew = sigmoid_fast(zf) * cprev + sigmoid_fast(zi) * tanh_fast(zg);
     hn = sigmoid_fast(zo) * tanh_fast(cnew);
-  } else if (gate_mode == kGatesExp) {
+  } else if constexpr (GM == kGatesExp) {
     cnew = sigmoid_acc(zf) * cprev + sigmoid_acc(zi) * tanh_acc(zg);
     hn = sigmoid_acc(zo) * tanh_acc(cnew);
   } else {
-    cnew = sigmoid_ieee(zf) * cprev + sigmoid_ieee(zi) * tanh_ieee(zg);
+    // the contraction is spelled out: f c rounded, i g fused onto it (left to the compiler, the choice of which
+    // product to fuse depends on the surrounding code, and the fp32 mode's outputs would change bits)
+    cnew = fmaf(sigmoid_ieee(zi), tanh_ieee(zg), __fmul_rn(sigmoid_ieee(zf), cprev));
     hn = sigmoid_ieee(zo) * tanh_ieee(cnew);
   }
 }
@@ -62,9 +65,10 @@ __device__ __forceinline__ void red_add_v4_f32(float* p, float4 v) {
                : "memory");
 }
 // po: offset of the first of the four units in the [row, out_pad] accumulator arrays (a multiple of 4); tg: global
-// timestep; len: valid length of the row
+// timestep; len: valid length of the row; mprev: the running max before this step if the caller already loaded it
+// (read from L2 after the (t-1, batch) counter was seen), nullptr to load it here
 __device__ __forceinline__ void pool_accumulate4(float* pool_sum, float* pool_max, float* pool_last, long long po,
-                                                 float4 hn, int tg, int len) {
+                                                 float4 hn, int tg, int len, const float4* mprev = nullptr) {
   if (tg >= len) return;
   float4* mp = reinterpret_cast<float4*>(pool_max + po);
   if (tg == 0) {
@@ -72,7 +76,7 @@ __device__ __forceinline__ void pool_accumulate4(float* pool_sum, float* pool_ma
     __stcg(mp, hn);
   } else {
     red_add_v4_f32(pool_sum + po, hn);
-    const float4 m = __ldcg(mp);
+    const float4 m = mprev != nullptr ? *mprev : __ldcg(mp);
     __stcg(mp, make_float4(fmaxf(m.x, hn.x), fmaxf(m.y, hn.y), fmaxf(m.z, hn.z), fmaxf(m.w, hn.w)));
   }
   if (tg == len - 1) __stcg(reinterpret_cast<float4*>(pool_last + po), hn);

@@ -49,7 +49,14 @@ constexpr int kLRows = 128;             // batch rows per item
 constexpr uint32_t kHBytes = kLRows * 64 * 2;
 constexpr uint32_t kWBytes = kLTileN * 64 * 2;
 constexpr uint32_t kStageBytes = kHBytes + kWBytes;
-constexpr int kGxPrefetchAhead = 8;     // k-blocks before the end of an item's MMAs at which its Gx lines are prefetched
+// k-blocks before the end of an item's MMAs at which each consumer thread loads its epilogue inputs into registers
+// (c_{t-1}, one row of fp16 Gx, the pooled layer's running max) and prefetches the rest of its Gx lines into L2
+constexpr int kEarlyLoadAhead = 8;
+// setmaxnreg budgets: the launch gives every thread 168 (65 536 / 384, rounded down to a multiple of 8); warpgroup 0
+// keeps 40, the two consumer warpgroups take the difference: 128 x 40 + 256 x 232 = 64 512 = 384 x 168
+constexpr uint32_t kProducerRegs = 40;
+constexpr uint32_t kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 384 * 168, "setmaxnreg budgets exceed the launch's registers");
 
 __device__ __forceinline__ void st_release_cta(uint32_t* p, uint32_t v) {
   asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
@@ -88,7 +95,7 @@ struct KArgs {
   long long ldy, raw_ld;
   long long* trace;
   long long* diag;
-  int T, t_begin, t0, T_total, ng, tiles, out_pad, nkb, segs, kh_pad, gate_mode, trace_items, fault;
+  int T, t_begin, t0, T_total, ng, tiles, out_pad, nkb, segs, kh_pad, trace_items, fault;
   int pre_nkb;           // FUSE: k-blocks of the input projection that precede the recurrent ones in every item
 };
 
@@ -106,7 +113,7 @@ struct KArgs {
 //     timestep leave most CTAs waiting on the step chain: the independent W_ih k-blocks run inside that wait.  The sum
 //     W_ih x + W_hh h + b stays in f32 (no fp16 rounding of Gx), so the fused layer is slightly MORE accurate than the
 //     hoisted form, but its bits differ from the hoisted form's (tests compare those two with IE_FUSE_LAST=0).
-template <bool TOK, bool GXBF, bool POOL, bool MC, bool FUSE>
+template <bool TOK, bool GXBF, bool POOL, bool MC, bool FUSE, int GM>
 __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const CUtensorMap& tm_w,
                                                 const CUtensorMap& tm_h64, const CUtensorMap& tm_x, const KArgs& a) {
   extern __shared__ uint8_t smem_raw[];
@@ -171,6 +178,8 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
   else __syncthreads();
 
   if (warp < 4) {
+    // warpgroup 0 is three single-lane loops and an idle warp: all 128 threads hand their registers to the consumers
+    setmaxnreg_dec<kProducerRegs>();
     if (warp == 0 && lane == 0) {
       // ---------------- h producer ------------------------------------------------------------------------------
       int stage = 0;
@@ -238,6 +247,7 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
   } else {
     // ---------------- consumers: MMA + epilogue (never leave their loop early: named barriers inside; in drain mode
     //                  their waits return at once and they run through the remaining items) ------------------------
+    setmaxnreg_inc<kConsumerRegs>();
     const int wg = (warp - 4) >> 2;              // which 64 rows of the item
     const int q = lane & 3;
     const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -252,8 +262,21 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
       int t, g, half, j;
       decode(n, t, g, half, j);
       const int tg = a.t0 + t;  // global timestep
+      const int brow0 = g * 256 + half * kLRows + rbase;   // this thread's rows: brow0 + 8 hr, hr = 0, 1
+      const int unit0 = j * 64 + 4 * q;                    // + 16 s: this thread's units of group s are unit0 + 16 s + 0..3
+      // Gx row of each of the two rows; TOK: a row of the per-token projection table, the token id loaded here at the
+      // item's start (its latency passes under the MMAs instead of stalling their issue at the early-load point)
+      long long grow[2];
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr)
+        grow[hr] = TOK ? static_cast<long long>(__ldg(a.tok + static_cast<long long>(tg) * b_pad + brow0 + 8 * hr))
+                       : static_cast<long long>(t) * b_pad + brow0 + 8 * hr;
+      // epilogue inputs loaded during the last MMAs (see kEarlyLoadAhead); c of both rows, pooled max (FUSE + POOL),
+      // fp16 Gx of row hr = 0 in gv (row hr = 1 is loaded into gv by the epilogue once row 0 is done)
+      float4 cv[2][4], mv[2][4];
+      uint4 gv[4][2];
       int prev = -1;
-      const int kb_prefetch = max(pre + nkt - kGxPrefetchAhead, 0);
+      const int kb_early = max(pre + nkt - kEarlyLoadAhead, pre);
       for (int kb = 0; kb < pre + nkt; ++kb) {
         mbar_wait(&full[stage], phase, ab);
         if (kb == pre && signal && wg == 0) IE_TRACE(2, k);          // first h_{t-1} stage landed
@@ -264,24 +287,47 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) wgmma_m64n256k16(d, da + 2 * kk, db + 2 * kk, (kb | kk) != 0);
         wgmma_commit();
-        if constexpr (!FUSE && !TOK) {
-          // Gx rows of this item come from HBM (a layer's Gx is streamed once, far larger than L2): pull the lines this
-          // thread's epilogue will read into L2 a few k-blocks before the MMAs end, so that the epilogue's dependent
-          // load -> store groups wait on L2 instead of HBM round trips.  Not earlier: lines held in L2 through the
-          // whole MMA phase compete with the weight k-blocks.  Not for TOK: its row index is a token id that would
-          // have to be loaded first, and that load stalls the MMA issue (measured slower).  Lane q of a quad takes
-          // line q (fp16: 4 lines of 128 B per row tile; f32: 8).
-          if (kb == kb_prefetch) {
+        if (kb == kb_early) {
+          // While the last k-blocks are on the tensor cores, load what the epilogue reads into registers (other than
+          // the accumulators), so that the epilogue is gate math and stores instead of a chain of L2 / HBM round
+          // trips.  Not earlier: Gx is streamed once from HBM, and lines held in L2 through the whole MMA phase
+          // compete with the weight k-blocks.
+          // c_{t-1} (and the running max) of this chain was written by another CTA: read it only after (t-1, g) has
+          // been seen here.  Already true: the h producer waited for the same count before loading the h stages
+          // these MMAs read.  In drain mode the loads may return stale values; the addresses stay in range.
+          if (lane == 0) wait_seq_ge(cready, static_cast<uint32_t>(k + 1), ab);
+          __syncwarp();
 #pragma unroll
-            for (int hr = 0; hr < 2; ++hr) {
-              const int brow = g * 256 + half * kLRows + rbase + 8 * hr;
-              const long long gtile = (static_cast<long long>(t) * b_pad + brow) * (4ll * a.out_pad) + j * kLTileN;
-              if constexpr (GXBF) {
-                prefetch_l2(reinterpret_cast<const __half*>(a.gx) + gtile + 64 * q);
-              } else {
-                prefetch_l2(reinterpret_cast<const float*>(a.gx) + gtile + 32 * q);
-                prefetch_l2(reinterpret_cast<const float*>(a.gx) + gtile + 32 * q + 128);
-              }
+          for (int hr = 0; hr < 2; ++hr) {
+            const long long co = static_cast<long long>(brow0 + 8 * hr) * a.out_pad + unit0;
+#pragma unroll
+            for (int s = 0; s < 4; ++s) {
+              cv[hr][s] = (tg == 0) ? make_float4(0.0f, 0.0f, 0.0f, 0.0f)
+                                    : __ldcg(reinterpret_cast<const float4*>(a.cstate + co + 16 * s));
+              if constexpr (FUSE && POOL)
+                mv[hr][s] = (tg == 0) ? make_float4(0.0f, 0.0f, 0.0f, 0.0f)
+                                      : __ldcg(reinterpret_cast<const float4*>(a.pool_max + co + 16 * s));
+            }
+          }
+          // Gx lines (fragment order, kernels.h frag_index): fp16 -- row 0 into registers, 16-byte chunk k of the
+          // thread's run at chunk position 4k + q; row 1 prefetched into L2, lane q of a quad taking line q of the
+          // row's 4 lines of 128 B.  f32 -- both rows prefetched, 8 lines per row.
+          if constexpr (!FUSE) {
+            const long long gtile0 = grow[0] * (4ll * a.out_pad) + j * kLTileN;
+            const long long gtile1 = grow[1] * (4ll * a.out_pad) + j * kLTileN;
+            if constexpr (GXBF) {
+              const uint4* gp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(a.gx) + gtile0) + q;
+#pragma unroll
+              for (int s = 0; s < 4; ++s)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) gv[s][i] = __ldcs(gp + 4 * (2 * s + i));
+              prefetch_l2(reinterpret_cast<const __half*>(a.gx) + gtile1 + 64 * q);
+            } else {
+              const float* gf = reinterpret_cast<const float*>(a.gx);
+              prefetch_l2(gf + gtile0 + 32 * q);
+              prefetch_l2(gf + gtile0 + 32 * q + 128);
+              prefetch_l2(gf + gtile1 + 32 * q);
+              prefetch_l2(gf + gtile1 + 32 * q + 128);
             }
           }
         }
@@ -302,44 +348,39 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
         if (MC) mbar_arrive_remote(&empty[prev], crank ^ 1u);
       }
       if (signal && wg == 0) IE_TRACE(3, k);
-      // c_{t-1} of this chain was written by another CTA: read it (from L2) only after (t-1, g) has been seen here
-      if (lane == 0) wait_seq_ge(cready, static_cast<uint32_t>(k + 1), ab);
-      __syncwarp();
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
-        const int brow = g * 256 + half * kLRows + rbase + 8 * hr;
+        const int brow = brow0 + 8 * hr;
         const int len = POOL ? a.lengths[brow] : 1;
-        const long long grow = TOK ? static_cast<long long>(__ldg(a.tok + static_cast<long long>(tg) * b_pad + brow))
-                                   : static_cast<long long>(t) * b_pad + brow;  // TOK: per-token projection table
-        const int unit0 = j * 64 + 4 * q;     // + 16 s: this thread's units of group s are unit0 + 16 s + 0..3
         float* cp = a.cstate + static_cast<long long>(brow) * a.out_pad + unit0;
         __nv_bfloat16* yrow = a.y + (static_cast<long long>(t + 1) * b_pad + brow) * a.ldy + unit0;
         const long long po = static_cast<long long>(brow) * a.out_pad + unit0;
         // this thread's run of 64 Gx values (or bias values) in the row's fragment-ordered tile: 16-byte chunk k at
         // chunk position 4k + q (kernels.h frag_index)
-        const long long gtile = grow * (4ll * a.out_pad) + j * kLTileN;
+        const long long gtile = grow[hr] * (4ll * a.out_pad) + j * kLTileN;
+        // fp16 Gx of row 1: all eight chunks issued before any of the row's stores (the compiler cannot move a load
+        // above a store it may alias), into the registers row 0's Gx has left; L2 hits after the prefetch
+        if constexpr (GXBF && !FUSE) {
+          if (hr == 1) {
+            const uint4* gp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(a.gx) + gtile) + q;
+#pragma unroll
+            for (int s = 0; s < 4; ++s)
+#pragma unroll
+              for (int i = 0; i < 2; ++i) gv[s][i] = __ldcs(gp + 4 * (2 * s + i));
+          }
+        }
         // FUSE: the bias tile in the same order; the empty asm makes its address opaque per row, so that the compiler
         // does not hoist the row-invariant bias loads out of the row loop (64 values held across it would spill)
         const float* btile = FUSE ? a.bias + j * kLTileN : nullptr;
         if constexpr (FUSE) asm volatile("" : "+l"(btile));
-        // the 16 units run in groups of four (one 16-byte c access, one 8-byte h store each): a group's loads (Gx or
-        // bias, c_{t-1}) are all issued before its stores, so their latencies overlap -- loads after the previous
-        // group's stores would be a chain of dependent L2 / HBM round trips per item (the compiler cannot move a load
-        // above a store it may alias)
+        // the 16 units run in groups of four (one 16-byte c access, one 8-byte h store each)
 #pragma unroll
         for (int s = 0; s < 4; ++s) {
           // accumulator chunk m = 4s + e holds unit 16s + 4q + e: (i, f) at d[8m + 2hr (+1)], (g, o) at d[8m + 4 + 2hr (+1)]
-          // Gx of the group's units e = 0..3, as loaded: fp16 -- two chunks of (i, f, g, o) x 2 units, issued here and
-          // widened only where they are added; f32 Gx and the bias (FUSE) -- one chunk of (i, f, g, o) per unit, loaded
-          // next to its use (four float4 in flight here would spill)
-          uint4 gh[2];
-          if constexpr (GXBF && !FUSE) {
-            const uint4* gp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(a.gx) + gtile) + q;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) gh[i] = __ldcs(gp + 4 * (2 * s + i));
-          }
-          const float4 cprev = (tg == 0) ? make_float4(0.0f, 0.0f, 0.0f, 0.0f)
-                                         : __ldcg(reinterpret_cast<const float4*>(cp + 16 * s));
+          // Gx of the group's units e = 0..3, as loaded: fp16 -- two chunks of (i, f, g, o) x 2 units, widened only
+          // where they are added; f32 Gx and the bias (FUSE) -- one chunk of (i, f, g, o) per unit, loaded next to its
+          // use
+          const float4 cprev = cv[hr][s];
           const float cp4[4] = {cprev.x, cprev.y, cprev.z, cprev.w};
           float cn[4], hn[4];
 #pragma unroll
@@ -349,6 +390,7 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
             if constexpr (FUSE) {
               gx = __ldg(reinterpret_cast<const float4*>(btile) + q + 4 * m);
             } else if constexpr (GXBF) {
+              const uint4* gh = gv[s];
               const uint32_t w0 = (e & 1) ? gh[e >> 1].z : gh[e >> 1].x, w1 = (e & 1) ? gh[e >> 1].w : gh[e >> 1].y;
               const float2 f01 = __half22float2(*reinterpret_cast<const __half2*>(&w0));
               const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&w1));
@@ -360,14 +402,15 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
             const float zf = d[8 * m + 2 * hr + 1] + gx.y;
             const float zg = d[8 * m + 4 + 2 * hr] + gx.z;
             const float zo = d[8 * m + 4 + 2 * hr + 1] + gx.w;
-            lstm_cell1(zi, zf, zg, zo, cp4[e], cn[e], hn[e], a.gate_mode);
+            lstm_cell1<GM>(zi, zf, zg, zo, cp4[e], cn[e], hn[e]);
           }
           const float4 h4 = make_float4(hn[0], hn[1], hn[2], hn[3]);
           __stcg(reinterpret_cast<float4*>(cp + 16 * s), make_float4(cn[0], cn[1], cn[2], cn[3]));
           store_h4(yrow + 16 * s, h4, lo_off);
           if (a.raw != nullptr)
             *reinterpret_cast<float4*>(a.raw + (static_cast<long long>(brow) * a.T_total + tg) * a.raw_ld + unit0 + 16 * s) = h4;
-          if constexpr (POOL) pool_accumulate4(a.pool_sum, a.pool_max, a.pool_last, po + 16 * s, h4, tg, len);
+          if constexpr (POOL)
+            pool_accumulate4(a.pool_sum, a.pool_max, a.pool_last, po + 16 * s, h4, tg, len, FUSE ? &mv[hr][s] : nullptr);
         }
       }
       // publish (step t, batch g): h_t / c_t / pooling state visible
@@ -395,39 +438,39 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
 
 thread_local int g_last_max_ctas = 0;   // result of the last check_only query on this thread
 
-template <bool TOK, bool GXBF, bool POOL>
+template <bool TOK, bool GXBF, bool POOL, int GM>
 __global__ void __launch_bounds__(kLThreads, 1)
 lstm_layer_kernel(const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_w,
                   const __grid_constant__ CUtensorMap tm_h64, const __grid_constant__ CUtensorMap tm_x,
                   const __grid_constant__ KArgs a) {
-  lstm_layer_body<TOK, GXBF, POOL, false, false>(tm_h, tm_w, tm_h64, tm_x, a);
+  lstm_layer_body<TOK, GXBF, POOL, false, false, GM>(tm_h, tm_w, tm_h64, tm_x, a);
 }
 
 // input projection fused into the K loop (the last layer by default; see FUSE above)
-template <bool POOL>
+template <bool POOL, int GM>
 __global__ void __launch_bounds__(kLThreads, 1)
 lstm_layer_fused_kernel(const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_w,
                         const __grid_constant__ CUtensorMap tm_h64, const __grid_constant__ CUtensorMap tm_x,
                         const __grid_constant__ KArgs a) {
-  lstm_layer_body<false, true, POOL, false, true>(tm_h, tm_w, tm_h64, tm_x, a);
+  lstm_layer_body<false, true, POOL, false, true, GM>(tm_h, tm_w, tm_h64, tm_x, a);
 }
 
-template <bool TOK>
+template <bool TOK, int GM>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kLThreads, 1)
 lstm_layer_mc_kernel(const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_w,
                      const __grid_constant__ CUtensorMap tm_h64, const __grid_constant__ CUtensorMap tm_x,
                      const __grid_constant__ KArgs a) {
-  lstm_layer_body<TOK, true, false, true, false>(tm_h, tm_w, tm_h64, tm_x, a);
+  lstm_layer_body<TOK, true, false, true, false, GM>(tm_h, tm_w, tm_h64, tm_x, a);
 }
 
 size_t layer_smem_bytes() { return 1024 + static_cast<size_t>(kLStages) * kStageBytes + 2 * kLStages * 8 + 32; }
 
-template <bool TOK, bool GXBF, bool POOL, bool MC, bool FUSE = false>
+template <int GM, bool TOK, bool GXBF, bool POOL, bool MC, bool FUSE = false>
 cudaError_t launch_layer_t(const LstmLayerArgs& a, int ctas, int tiles, cudaStream_t stream) {
   void (*kfn)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, KArgs);
-  if constexpr (MC) kfn = lstm_layer_mc_kernel<TOK>;
-  else if constexpr (FUSE) kfn = lstm_layer_fused_kernel<POOL>;
-  else kfn = lstm_layer_kernel<TOK, GXBF, POOL>;
+  if constexpr (MC) kfn = lstm_layer_mc_kernel<TOK, GM>;
+  else if constexpr (FUSE) kfn = lstm_layer_fused_kernel<POOL, GM>;
+  else kfn = lstm_layer_kernel<TOK, GXBF, POOL, GM>;
   const size_t smem = layer_smem_bytes();
   // function attributes are per device: set on every launch (cheap), never cached in a process-wide flag
   cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -462,7 +505,7 @@ cudaError_t launch_layer_t(const LstmLayerArgs& a, int ctas, int tiles, cudaStre
   k.ldy = a.ldy; k.raw_ld = a.raw_ld; k.trace = a.trace; k.diag = a.diag;
   k.T = a.single_step ? 1 : a.T; k.t_begin = a.single_step ? a.t_step : 0;
   k.t0 = a.t0; k.T_total = a.T_total; k.ng = a.ng; k.tiles = tiles; k.out_pad = a.out_pad;
-  k.nkb = a.kh_pad / 64; k.segs = a.segs; k.kh_pad = a.kh_pad; k.gate_mode = a.gate_mode;
+  k.nkb = a.kh_pad / 64; k.segs = a.segs; k.kh_pad = a.kh_pad;
   k.trace_items = a.trace_items; k.fault = a.fault;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(ctas);
@@ -502,29 +545,43 @@ int lstm_layer_ctas(const LstmLayerArgs& a) {
   return static_cast<int>(ctas);
 }
 
-// a.check_only: only query co-residency (lstm_layer_max_ctas()).  Requires u == 32 per slice (64 units per tile).
-cudaError_t launch_lstm_layer(const LstmLayerArgs& a, cudaStream_t stream) {
+namespace {
+
+template <int GM>
+cudaError_t launch_lstm_layer_gm(const LstmLayerArgs& a, cudaStream_t stream) {
   if (a.u != 32 || a.n_cta % 2 || a.kh_pad % 64 || a.ng < 1 || a.ng > kMaxBatches || a.T < 1 || (a.segs != 1 && a.segs != 3))
     return cudaErrorInvalidValue;
   const int tiles = a.n_cta / 2;
-  if (a.check_only && a.mc) return launch_layer_t<false, true, false, true>(a, 0, tiles, stream);
+  if (a.check_only && a.mc) return launch_layer_t<GM, false, true, false, true>(a, 0, tiles, stream);
   const int ctas = lstm_layer_ctas(a);
   if (ctas < 1) return cudaErrorInvalidValue;
   const bool tok = a.tok != nullptr;  // layer 0 reading its input projection from the per-token table
   const bool pool = a.pool_sum != nullptr;
   if (a.pre_nkb > 0) {  // input projection fused into the K loop: tm_w covers [W_ih | W_hh], tm_x the previous layer's ring
     if (a.check_only || tok || a.segs != 1 || a.bias == nullptr || a.single_step) return cudaErrorInvalidValue;
-    return pool ? launch_layer_t<false, true, true, false, true>(a, ctas, tiles, stream)
-                : launch_layer_t<false, true, false, false, true>(a, ctas, tiles, stream);
+    return pool ? launch_layer_t<GM, false, true, true, false, true>(a, ctas, tiles, stream)
+                : launch_layer_t<GM, false, true, false, false, true>(a, ctas, tiles, stream);
   }
   if (!a.check_only && lstm_layer_mc_ok(a))
-    return tok ? launch_layer_t<true, true, false, true>(a, ctas, tiles, stream)
-               : launch_layer_t<false, true, false, true>(a, ctas, tiles, stream);
+    return tok ? launch_layer_t<GM, true, true, false, true>(a, ctas, tiles, stream)
+               : launch_layer_t<GM, false, true, false, true>(a, ctas, tiles, stream);
 #define IE_LAYER(T_, G_)                                                                                  \
-  (pool ? launch_layer_t<T_, G_, true, false>(a, ctas, tiles, stream) : launch_layer_t<T_, G_, false, false>(a, ctas, tiles, stream))
+  (pool ? launch_layer_t<GM, T_, G_, true, false>(a, ctas, tiles, stream) : launch_layer_t<GM, T_, G_, false, false>(a, ctas, tiles, stream))
   if (a.gx_bf16) return tok ? IE_LAYER(true, true) : IE_LAYER(false, true);
   return tok ? IE_LAYER(true, false) : IE_LAYER(false, false);
 #undef IE_LAYER
+}
+
+}  // namespace
+
+// a.check_only: only query co-residency (lstm_layer_max_ctas()).  Requires u == 32 per slice (64 units per tile).
+cudaError_t launch_lstm_layer(const LstmLayerArgs& a, cudaStream_t stream) {
+  switch (a.gate_mode) {   // compiled per gate mode (lstm_common.cuh lstm_cell1)
+    case kGatesFast: return launch_lstm_layer_gm<kGatesFast>(a, stream);
+    case kGatesExp: return launch_lstm_layer_gm<kGatesExp>(a, stream);
+    case kGatesIeee: return launch_lstm_layer_gm<kGatesIeee>(a, stream);
+    default: return cudaErrorInvalidValue;
+  }
 }
 
 }  // namespace ie

@@ -80,12 +80,13 @@ __device__ __forceinline__ bool aborted(const Abort& a) {
   asm volatile("ld.volatile.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(smem_u32(a.s)) : "memory");
   return v != 0;
 }
-static __device__ __noinline__ void abort_raise(const Abort& a) {
+// Inlined, like every helper here: an out-of-line (ABI) call in a kernel makes ptxas ignore its setmaxnreg budgets.
+static __device__ __forceinline__ void abort_raise(const Abort& a) {
   asm volatile("st.volatile.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(a.s)), "r"(1u) : "memory");
   if (a.g != nullptr) atomicExch(a.g, 1u);
 }
 // slow-path poll (every few hundred spins): true once this CTA is in drain mode
-static __device__ __noinline__ bool abort_poll(const Abort& a, long long t0) {
+static __device__ __forceinline__ bool abort_poll(const Abort& a, long long t0) {
   if (aborted(a)) return true;
   bool hit = (clock64() - t0) > a.limit;
   if (!hit && a.g != nullptr) {
@@ -240,6 +241,15 @@ __device__ __forceinline__ void prefetch_l2(const void* p) {
 }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// per-thread register budget of the executing warpgroup from here on (every thread of all four warps must execute the
+// same instruction): producer warpgroups give registers back to the SM's pool, consumer warpgroups take them
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 
 // ----------------------------------------------------------------------------------------------

@@ -156,10 +156,15 @@ class IssueEncoder:
         check(self._lib.ie_encoder_raw_features(self._h, ids.ctypes.data, B, T, raw.ctypes.data, 0, None))
         return raw
 
-    def _debug_layer_states(self, layer: int, ids) -> np.ndarray:
+    def _debug_layer_states(self, layer: int, ids):
         """Test hook ``ie_debug_layer_states``: hidden states of ``layer`` (B, T, out_l) float32 as its recurrent kernel
-        computed them (the ring holds their bf16 rounding); for the last layer identical to ``raw_features``."""
-        ids = np.ascontiguousarray(np.asarray(ids.cpu() if hasattr(ids, "cpu") else ids), dtype=np.int64)
+        computed them (the ring holds their bf16 rounding); for the last layer identical to ``raw_features``.
+        Host ids give a numpy array.  CUDA int64 ids give a CUDA tensor written in place on torch's current stream
+        (IE_FLAG_DEVICE_PTRS: nothing passes through host memory, where one 1280 x 512 x 2400 layer takes 6.3 GB);
+        ``check_errors()`` reports that call's data-dependent errors."""
+        on_device = getattr(ids, "is_cuda", False)
+        if not on_device:
+            ids = np.ascontiguousarray(np.asarray(ids.cpu() if hasattr(ids, "cpu") else ids), dtype=np.int64)
         if ids.ndim != 2:
             raise ValueError("ids must be (B, T)")
         B, T = ids.shape
@@ -168,6 +173,16 @@ class IssueEncoder:
         if not 0 <= layer < self.n_layers:
             raise ValueError(f"layer {layer} outside [0, {self.n_layers})")
         out_l = self.emb_sz if layer == self.n_layers - 1 else self.n_hid
+        if on_device:
+            import torch
+            if ids.dtype != torch.int64:
+                raise ValueError("device ids must be int64")
+            ids = ids.contiguous()
+            out = torch.empty((B, T, out_l), dtype=torch.float32, device=ids.device)
+            s = torch.cuda.current_stream(ids.device)
+            check(self._lib.ie_debug_layer_states(self._h, layer, ids.data_ptr(), B, T, out.data_ptr(),
+                                                  IE_FLAG_DEVICE_PTRS, C.c_void_p(s.cuda_stream)))
+            return out
         out = np.empty((B, T, out_l), dtype=np.float32)
         check(self._lib.ie_debug_layer_states(self._h, layer, ids.ctypes.data, B, T, out.ctypes.data, 0, None))
         return out

@@ -30,7 +30,11 @@ torch device the inputs live on); only the float64 cell-state recursion is seque
 e_c,t = f_t e_c,t-1 + ... because the device's cell state is not observed.
 
 Mutants (``Mode`` fields and ``pool(..., mutant=)``) are deliberately wrong variants of the arithmetic; tests use them
-as negative controls that the bound must reject.
+as negative controls that the bound must reject.  Some apply at every step (a wrong rounding point, a permutation slip);
+the ``*_at`` ones touch a single step of a few units, which is what a broken schedule does to one work item.
+
+``blocked_layer_stats`` runs the teacher-forced check over every row of a benchmark-size launch a block of rows at a
+time and reduces it to the statistics the tests cap, with the largest ratio of every schedule item of lstm_layer.cu.
 """
 from __future__ import annotations
 
@@ -134,13 +138,18 @@ class Mode:
     """Arithmetic of one layer.  segs: 0 exact f64 operands, 1 bf16, 3 split-bf16.  gx: 'fp16' | 'f32' | 'fused' |
     'exact' (mutant: 'bf16').  gates: 'fast' | 'exp' | 'ieee' | 'exact'.  cell: 'f32' | 'exact' (mutant: 'bf16').
     Mutants: stale_c -- units that read c_{t-2} instead of c_{t-1} (a lost-ordering race); swap_fo -- units whose f and o
-    gates are exchanged (a permutation slip)."""
+    gates are exchanged (a permutation slip).  Confined to one step (t, units): stale_c_at -- at step t the units read
+    c_{t-2}; stale_h_at -- at step t the z of the units is formed from h_{t-2} (a ring slot read before it was written);
+    carry_lost_at = t0 -- at step t0 h_{t0-1} and c_{t0-1} read as zero (a lost time-chunk carry)."""
     segs: int = 1
     gx: str = "fp16"
     gates: str = "fast"
     cell: str = "f32"
     stale_c: tuple = ()
     swap_fo: tuple = ()
+    stale_c_at: tuple = ()
+    stale_h_at: tuple = ()
+    carry_lost_at: int = -1
 
 
 EXACT = Mode(segs=0, gx="exact", gates="exact", cell="exact")
@@ -208,7 +217,8 @@ def _gate_views(z: torch.Tensor, H: int, swap_fo=()):
 
 
 def _cell_loop(z, ez, H, mode: Mode, T: int):
-    """Gates and the sequential f64 cell recursion over t of z [R, T, 4H] -> (h [R, T, H], bound [R, T, H])."""
+    """Gates and the sequential f64 cell recursion over t of z [R, T, 4H] -> (h [R, T, H], bound [R, T, H]).  Only c
+    and its error bound e_c are sequential; everything else runs over all steps at once."""
     zi, zf, zg, zo = _gate_views(z, H, mode.swap_fo)
     ei, ef, eg_, eo = _gate_views(ez, H, mode.swap_fo)
     k = mode.gates
@@ -217,29 +227,36 @@ def _cell_loop(z, ez, H, mode: Mode, T: int):
     ef = f * (1 - f) * ef + sig_err(zf, f, k)
     eo = o * (1 - o) * eo + sig_err(zo, o, k)
     eg_ = (1 - g * g) * eg_ + tanh_err(zg, g, k)
+    rnd = mode.cell != "exact"
+    ig = i * g
+    e_ig = g.abs() * ei + i.abs() * eg_ + (U24 * ig.abs() if rnd else 0)
+    del ei, eg_
     R = z.shape[0]
     c1 = torch.zeros(R, H, dtype=z.dtype, device=z.device)   # c_{t-1}
-    c2 = torch.zeros_like(c1)                                   # c_{t-2} (stale-read mutant)
+    c2 = torch.zeros_like(c1)                                   # c_{t-2} (stale-read mutants)
     ec = torch.zeros_like(c1)
-    hs, eh = torch.empty(R, T, H, dtype=z.dtype, device=z.device), torch.empty(R, T, H, dtype=z.dtype, device=z.device)
-    rnd = mode.cell != "exact"
+    cs, ecs = torch.empty_like(ig), torch.empty_like(ig)
     for t in range(T):
         cp = c1
         if mode.stale_c:
             cp = c1.clone()
             cp[:, list(mode.stale_c)] = c2[:, list(mode.stale_c)]
-        ig = i[:, t] * g[:, t]
-        c = f[:, t] * cp + ig                                   # lstm_common.cuh lstm_cell1: cnew = f c + i g (f32)
+        if mode.stale_c_at and mode.stale_c_at[0] == t:
+            cp = c1.clone()
+            cp[:, list(mode.stale_c_at[1])] = c2[:, list(mode.stale_c_at[1])]
+        if mode.carry_lost_at == t:
+            cp = torch.zeros_like(c1)
+        c = torch.addcmul(ig[:, t], f[:, t], cp)               # lstm_common.cuh lstm_cell1: cnew = f c + i g (f32)
         if mode.cell == "bf16":
             c = rne_bf16(c)
-        ec = (f[:, t] * ec + cp.abs() * ef[:, t] + g[:, t].abs() * ei[:, t] + i[:, t].abs() * eg_[:, t]
-              + (U24 * (ig.abs() + c.abs()) if rnd else 0))
-        tc = torch.tanh(c)
-        h = o[:, t] * tc                                        # hn = o tanh(cnew)
-        hs[:, t] = h
-        eh[:, t] = (tc.abs() * eo[:, t] + o[:, t] * ((1 - tc * tc) * ec + tanh_err(c, tc, k))
-                    + (U24 * h.abs() if rnd else 0))
+        ec = torch.addcmul(e_ig[:, t], f[:, t], ec).addcmul_(cp.abs(), ef[:, t])
+        if rnd:
+            ec.add_(c.abs(), alpha=U24)
+        cs[:, t], ecs[:, t] = c, ec
         c2, c1 = c1, c
+    tc = torch.tanh(cs)
+    hs = o * tc                                                 # hn = o tanh(cnew)
+    eh = tc.abs() * eo + o * ((1 - tc * tc) * ecs + tanh_err(cs, tc, k)) + (U24 * hs.abs() if rnd else 0)
     return hs, eh
 
 
@@ -257,10 +274,21 @@ def teacher_forced_layer(x_in, h_dev, weights: dict, mode: Mode, acc_ulps: float
     x_in = _t(x_in, dev)
     R, T, H = h_dev.shape
     x = x_in.reshape(R * T, -1)
-    hprev = torch.cat([torch.zeros(R, 1, H, dtype=h_dev.dtype, device=dev), h_dev[:, :-1]], 1).reshape(R * T, H)
+    hprev = torch.cat([torch.zeros(R, 1, H, dtype=h_dev.dtype, device=dev), h_dev[:, :-1]], 1)
+    if mode.carry_lost_at >= 0:
+        hprev[:, mode.carry_lost_at] = 0
+    hprev = hprev.reshape(R * T, H)
     s = mode.segs
+    w_hh = _t(weights["w_hh"], dev)
     px, ax = products(operands(x, s), operands(_t(weights["w_ih"], dev), s), s)
-    ph, ah = products(operands(hprev, s), operands(_t(weights["w_hh"], dev), s), s)
+    ph, ah = products(operands(hprev, s), operands(w_hh, s), s)
+    if mode.stale_h_at:
+        t, units = mode.stale_h_at
+        cols = [q * H + u for q in range(4) for u in units]
+        h2 = h_dev[:, t - 2] if t >= 2 else torch.zeros_like(h_dev[:, 0])
+        p2, a2 = products(operands(h2, s), operands(w_hh[cols], s), s)
+        ph.view(R, T, 4 * H)[:, t, cols] = p2
+        ah.view(R, T, 4 * H)[:, t, cols] = a2
     z, ez = _preactivation(px, ax, ph, ah, _bias(weights, mode, dev), mode, acc_ulps)
     return _cell_loop(z.reshape(R, T, 4 * H), ez.reshape(R, T, 4 * H), H, mode, T)
 
@@ -398,3 +426,51 @@ def ratio_stats(h_dev, pred, bound) -> dict:
     h_dev = _t(h_dev, pred.device)
     r = (h_dev - pred).abs() / bound.clamp_min(1e-30)
     return {"max": float(r.max()), "rms": float(torch.sqrt((r * r).mean()))}
+
+
+ITEM_ROWS, ITEM_UNITS, BATCH_ROWS = 128, 64, 256   # lstm_layer.cu: kLRows rows x kLTileN / 4 units per item; one batch
+
+
+def item_of(row: int, unit: int):
+    """(batch g, row half, column tile j) of the schedule item that computes h[row, t, unit] at every step t."""
+    return row // BATCH_ROWS, (row % BATCH_ROWS) // ITEM_ROWS, unit // ITEM_UNITS
+
+
+def blocked_layer_stats(x_in, h_dev, weights: dict, mode: Mode, rows: range | None = None, block: int = 32,
+                        acc_ulps: float = ACC_ULPS) -> dict:
+    """teacher_forced_layer over `rows` (default: all) of one layer, `block` rows at a time, reduced to statistics of
+    r = |h_dev - pred| / bound (ratio_stats on every element, without holding the [R, T, 4H] float64 working set).
+
+    x_in [R, T, in], h_dev [R, T, out] as for teacher_forced_layer (any float dtype; the work runs on h_dev's device).
+    Returns max, rms, sumsq and n (so that statistics of several row sets combine), above_half (count of r > 0.5),
+    argmax (row, t, unit) and items: the largest r of every schedule item, float64 [T, ng, 2, tiles] indexed by
+    (t, batch g, row half, column tile j) as item_of maps rows and units (zero for items outside `rows`)."""
+    R, T, H = h_dev.shape
+    dev = h_dev.device
+    rows = range(R) if rows is None else rows
+    w = dict(weights, w_ih=_t(weights["w_ih"], dev), w_hh=_t(weights["w_hh"], dev))
+    ng, tiles = -(-R // BATCH_ROWS), -(-H // ITEM_UNITS)
+    items = torch.zeros(T, ng, 2, tiles, dtype=torch.float64, device=dev)
+    out = {"max": -1.0, "sumsq": 0.0, "n": 0, "above_half": 0, "argmax": None}
+    for r0 in range(rows.start, rows.stop, block):
+        r1 = min(r0 + block, rows.stop)
+        pred, bound = teacher_forced_layer(x_in[r0:r1], h_dev[r0:r1], w, mode, acc_ulps)
+        r = (_t(h_dev[r0:r1]) - pred).abs_().div_(bound.clamp_min_(1e-30))
+        del pred, bound
+        m = float(r.max())
+        if m > out["max"]:
+            k = int(r.argmax())
+            out["max"], out["argmax"] = m, (r0 + k // (T * H), (k // H) % T, k % H)
+        out["sumsq"] += float((r * r).sum())
+        out["n"] += r.numel()
+        out["above_half"] += int((r > 0.5).sum())
+        per_tile = torch.nn.functional.pad(r, (0, tiles * ITEM_UNITS - H)).view(r1 - r0, T, tiles, ITEM_UNITS).amax(3)
+        for q0 in range(r0, r1):   # rows of the block grouped by (batch, row half)
+            if q0 > r0 and q0 % ITEM_ROWS:
+                continue
+            q1 = min(r1, (q0 // ITEM_ROWS + 1) * ITEM_ROWS)
+            g, half, _ = item_of(q0, 0)
+            items[:, g, half] = torch.maximum(items[:, g, half], per_tile[q0 - r0:q1 - r0].amax(0))
+    out["rms"] = (out["sumsq"] / out["n"]) ** 0.5
+    out["items"] = items
+    return out

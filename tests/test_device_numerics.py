@@ -113,6 +113,61 @@ def test_layer_modes_follow_the_knobs():
     assert [m.gx for m in D.layer_modes(2)] == ["fp16", "fused"]
 
 
+def _small_layer(n_rows, T):
+    """Layer 0 of the small model (96 -> 200 units: four column tiles, the last one partial) on n_rows rows, states
+    from the float32 emulation."""
+    emb, layers = R.make_encoder(7, CFG[3], CFG[1], CFG[2], CFG[0], scale=2.0).export_weights()
+    ids = np.stack(R.synthetic_ids(n_rows, T, seed=5, vocab_sz=CFG[3]))
+    x = torch.from_numpy(emb[ids])
+    h = D.free_run_layer(x, layers[0], D.Mode(), torch.float32)
+    return x, h, layers[0]
+
+
+def test_blocked_statistics_equal_the_unblocked_ones():
+    """300 rows (two batches, the second one ending inside its first row half) in blocks of 48 rows, which straddle the
+    row-half boundaries at 128 and 256."""
+    x, h, w = _small_layer(300, 7)
+    pred, bound = D.teacher_forced_layer(x, h, w, D.Mode())
+    r = ((h - pred).abs() / bound.clamp_min(1e-30))
+    want = D.ratio_stats(h, pred, bound)
+    got = D.blocked_layer_stats(x, h, w, D.Mode(), block=48)
+    assert got["max"] == pytest.approx(want["max"], rel=1e-12) and got["rms"] == pytest.approx(want["rms"], rel=1e-12)
+    assert got["n"] == r.numel() and got["above_half"] == int((r > 0.5).sum())
+    assert got["argmax"] == tuple(int(v) for v in np.unravel_index(int(r.argmax()), r.shape))
+    items = got["items"]
+    assert items.shape == (7, 2, 2, 4)
+    for g, half, j in np.ndindex(2, 2, 4):
+        rows = r[g * 256 + half * 128:min(300, g * 256 + half * 128 + 128), :, j * 64:(j + 1) * 64]
+        want_item = rows.amax((0, 2)) if rows.shape[0] else torch.zeros(7, dtype=torch.float64)
+        torch.testing.assert_close(items[:, g, half, j], want_item, rtol=1e-12, atol=0)
+    # a row range: the statistics of rows 128..255 only, and nothing outside them
+    sub = D.blocked_layer_stats(x, h, w, D.Mode(), rows=range(128, 256), block=32)
+    assert sub["max"] == pytest.approx(float(r[128:256].max()), rel=1e-12)
+    assert sub["n"] == r[128:256].numel()
+    assert float(sub["items"][:, 0, 0].max()) == 0 and float(sub["items"][:, 1].max()) == 0
+    assert D.item_of(299, 199) == (1, 0, 3) and D.item_of(127, 64) == (0, 0, 1) and D.item_of(128, 63) == (0, 1, 0)
+
+
+@pytest.mark.parametrize("name", ["stale_c_at", "stale_h_at", "carry_lost_at"])
+def test_item_local_mutants_change_exactly_the_elements_they_name(name):
+    """A mutant confined to (step t, units of one tile) changes the prediction of those units from step t on (the cell
+    state carries the wrong value forward) and of nothing else; a lost carry at t0 changes every unit from t0 on.  Each
+    also breaks the bound there."""
+    x, h, w = _small_layer(40, 9)
+    t, units = 4, tuple(range(64, 128))
+    mutant = {"stale_c_at": D.Mode(stale_c_at=(t, units)), "stale_h_at": D.Mode(stale_h_at=(t, units)),
+              "carry_lost_at": D.Mode(carry_lost_at=t)}[name]
+    pred, bound = D.teacher_forced_layer(x, h, w, D.Mode())
+    pred_m, bound_m = D.teacher_forced_layer(x, h, w, mutant)
+    want = torch.zeros_like(pred, dtype=torch.bool)
+    want[:, t:, :] = True
+    if name != "carry_lost_at":
+        want[:, :, :64] = want[:, :, 128:] = False
+    assert torch.equal(pred_m != pred, want)
+    ratio = (h - pred_m).abs() / bound_m
+    assert float(ratio[:, t].max()) > 4 * float(((h - pred).abs() / bound).max())
+
+
 def test_pool_restates_the_kernel_and_mutants_differ():
     rng = np.random.default_rng(0)
     h = (rng.standard_normal((6, 9, 5)) * 0.3).astype(np.float32)

@@ -56,6 +56,7 @@ PROTOTYPES = {
     "ie_debug_gemm_frag": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_int32, C.c_void_p, C.c_int32]),
     "ie_debug_epilogue_layout": (C.c_int64, [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "ie_debug_gates": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),
     "ie_debug_layer_states": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                         C.c_void_p]),
     "ie_knn_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]),
@@ -117,6 +118,29 @@ def _debug_gemm(a, b, bias=None, act: int = 0, out_type: int = 0, segs: int = 1,
     check(load().ie_debug_gemm_ex(a.ctypes.data, b.ctypes.data, bias_p, M, N, K, act, out_type, segs, d.ctypes.data,
                                   device))
     return d
+
+
+GATE_FNS = ("sigmoid_fast", "tanh_fast", "sigmoid_acc", "tanh_acc", "sigmoid_ieee", "tanh_ieee")
+CELL_FNS = {"fast": 6, "exp": 7, "ieee": 8}
+
+
+def _debug_gates(fn, x):
+    """Test hook ``ie_debug_gates`` on CUDA float32 tensors.  fn a name of GATE_FNS: f(x) elementwise, same shape.
+    fn 'cell_fast' | 'cell_exp' | 'cell_ieee': x [5, n] planes (zi, zf, zg, zo, c_prev) -> [2, n] (c_new, h)."""
+    import torch
+    x = x.contiguous()
+    if x.dtype != torch.float32 or not x.is_cuda:
+        raise ValueError("ie_debug_gates takes a CUDA float32 tensor")
+    if fn in GATE_FNS:
+        code, n, out = GATE_FNS.index(fn), x.numel(), torch.empty_like(x)
+    else:
+        code = CELL_FNS[fn.removeprefix("cell_")]
+        if x.dim() != 2 or x.shape[0] != 5:
+            raise ValueError(f"cell input {tuple(x.shape)} must be [5, n]")
+        n, out = x.shape[1], torch.empty(2, x.shape[1], dtype=torch.float32, device=x.device)
+    stream = torch.cuda.current_stream(x.device).cuda_stream
+    check(load().ie_debug_gates(code, x.data_ptr(), out.data_ptr(), n, x.device.index, stream))
+    return out
 
 
 def check(rc: int) -> None:

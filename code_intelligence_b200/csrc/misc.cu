@@ -168,6 +168,36 @@ __global__ void fill_f32_kernel(float* p, size_t n, float v) {
   for (; i < n; i += stride) p[i] = v;
 }
 
+// test hook ie_debug_gates: the gate functions and the cell update exactly as the recurrent kernel and the GEMM
+// epilogue inline them (ptx.cuh, lstm_common.cuh)
+template <int FN>
+__global__ void debug_gate_kernel(const float* __restrict__ x, float* __restrict__ y, long long n) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const float v = x[i];
+    float r;
+    if constexpr (FN == 0) r = sigmoid_fast(v);
+    else if constexpr (FN == 1) r = tanh_fast(v);
+    else if constexpr (FN == 2) r = sigmoid_acc(v);
+    else if constexpr (FN == 3) r = tanh_acc(v);
+    else if constexpr (FN == 4) r = sigmoid_ieee(v);
+    else r = tanh_ieee(v);
+    y[i] = r;
+  }
+}
+
+// in = planes [zi | zf | zg | zo | c_prev] of n values, out = planes [c_new | h]
+template <int GM>
+__global__ void debug_cell_kernel(const float* __restrict__ in, float* __restrict__ out, long long n) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    float c, h;
+    lstm_cell1<GM>(in[i], in[n + i], in[2 * n + i], in[3 * n + i], in[4 * n + i], c, h);
+    out[i] = c;
+    out[n + i] = h;
+  }
+}
+
 }  // namespace
 
 cudaError_t launch_embed_gather(const int64_t* ids, int B, int T, int b_pad, const __nv_bfloat16* emb, int vocab,
@@ -221,6 +251,26 @@ cudaError_t launch_fill_f32(float* p, size_t n, float v, cudaStream_t stream) {
   size_t blocks = (n + 255) / 256;
   if (blocks > 132 * 16) blocks = 132 * 16;
   fill_f32_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(p, n, v);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_debug_gates(int fn, const float* in, float* out, long long n, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  long long blocks = (n + 255) / 256;
+  if (blocks > 132 * 64) blocks = 132 * 64;
+  const unsigned g = static_cast<unsigned>(blocks);
+  switch (fn) {
+    case 0: debug_gate_kernel<0><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 1: debug_gate_kernel<1><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 2: debug_gate_kernel<2><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 3: debug_gate_kernel<3><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 4: debug_gate_kernel<4><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 5: debug_gate_kernel<5><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 6: debug_cell_kernel<kGatesFast><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 7: debug_cell_kernel<kGatesExp><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 8: debug_cell_kernel<kGatesIeee><<<g, 256, 0, stream>>>(in, out, n); break;
+    default: return cudaErrorInvalidValue;
+  }
   return cudaGetLastError();
 }
 

@@ -183,6 +183,13 @@ int ie_debug_gemm_frag(const float* a, const float* b, const float* bias, int32_
  * receive the fragment-order position of each column of a 256-column tile for 2- and 4-byte elements. */
 int64_t ie_debug_epilogue_layout(int32_t out_units, int32_t* perm, int64_t cap, int32_t* frag2, int32_t* frag4);
 
+/* Debug / test hook, device pointers on `device`, asynchronous on `stream`: the gate functions and the cell update as the
+ * recurrent kernel and the GEMM epilogue compute them (the same inline device functions).
+ *   fn 0..5: out[i] = f(in[i]), i < n, f = sigmoid_fast, tanh_fast, sigmoid_acc, tanh_acc, sigmoid_ieee, tanh_ieee
+ *   fn 6, 7, 8: the cell update with fast, exp (IE_CFG_ACCURATE_GATES) or IEEE (IE_CFG_FP32) gates:
+ *   in = planes [zi | zf | zg | zo | c_prev] of n values each, out = planes [c_new | h]. */
+int ie_debug_gates(int32_t fn, const float* in, float* out, int64_t n, int32_t device, void* stream);
+
 /* Debug / test hook: the hidden states of layer `layer` of an encode of ids [B, T] (zero initial state), as that
  * layer's recurrent kernel computed them: out [B, T, out_l] f32, out_l = n_hid, or emb_sz for the last layer.  The
  * hidden-state ring the next step and the next layer read holds their bf16 round-to-nearest-even (hi + lo in the

@@ -15,10 +15,11 @@ import numpy as np
 U24 = 2.0 ** -24
 SPLIT_PRODUCT = 3.1 * 2.0 ** -18   # split-bf16 (hi*hi + lo*hi + hi*lo) vs the exact product, relative to |q~ x~|
 PASSES = 3                         # split-bf16 K loop: hi*hi, lo*hi, hi*lo into one f32 accumulator
-# f32 accumulation: one rounding of at most 2^-23 of the running sum (|.| <= sum |q~ x~|) per k16 MMA step, K_pad / 16
-# steps per pass.  The per-pass 8 * 2^-24 of the encoder's checks assumes sums far below sum |q~ x~|; centred
-# clustered data keeps the partial sums of a query's own cluster near sum |q~ x~|, where that is exceeded.
-ACC_STEP = 2.0 ** -23
+# f32 accumulation (oracle/tc_accum.py MODEL, measured on the H100): each k16 MMA step loses less than
+# 17 * 2^-25 of its largest term (C or a product) to alignment and 2^-23 of its result to the truncation to f32; every
+# such value is at most the sum of |split products|, <= (1 + 2^-6) sum |q~ x~|.  K_pad / 16 steps per pass.  (Centred
+# clustered data keeps the partial sums of a query's own cluster near sum |q~ x~|, so no per-pass constant holds.)
+ACC_STEP = 17 * 2.0 ** -25 + 2.0 ** -23
 
 
 def _exact(Q, X, cand, metric):
@@ -85,7 +86,7 @@ def stage1_scores(X, Q, c, metric):
     dot_t = Qt @ Xt.T
     abs_t = np.abs(Qt) @ np.abs(Xt).T
     k_pad = -(-X.shape[1] // 64) * 64
-    e_acc = (SPLIT_PRODUCT + PASSES * (k_pad // 16) * ACC_STEP) * abs_t
+    e_acc = (SPLIT_PRODUCT + PASSES * (k_pad // 16) * ACC_STEP * (1 + 2.0 ** -6)) * abs_t
     if metric == "euclidean":
         h = 0.5 * (Xt * Xt).sum(1)[None, :]
         s = dot_t - h

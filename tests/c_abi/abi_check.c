@@ -19,7 +19,7 @@ int main(void) {
                (fn)ie_encoder_launch_count, (fn)ie_encoder_max_batch, (fn)ie_encoder_last_phase_ms, (fn)ie_debug_seq_trace,
                (fn)ie_encoder_check_errors, (fn)ie_encoder_last_phase_mhz, (fn)ie_mlp_create, (fn)ie_mlp_load_layer, (fn)ie_mlp_predict_proba,
                (fn)ie_mlp_destroy, (fn)ie_pr_thresholds, (fn)ie_debug_gemm, (fn)ie_debug_gemm_ex,
-               (fn)ie_debug_layer_states};
+               (fn)ie_debug_layer_states, (fn)ie_debug_gates};
   memset(&cfg, 0, sizeof cfg);
   cfg.n_layers = 4; cfg.emb_sz = 800; cfg.n_hid = 2400; cfg.vocab_sz = 60000; cfg.pad_idx = 1;
   printf("version=%d symbols=%d max_batch=%d\n", ie_version(), (int)(sizeof syms / sizeof syms[0]), IE_MAX_BATCH);

@@ -207,3 +207,29 @@ def test_gemm_interval_and_mlp_head_contain_float32_emulations():
     _, lo, hi = D.mlp_head(a, coefs, ints)
     assert bool(((p32 >= lo) & (p32 <= hi)).all())
     np.testing.assert_allclose(D.mlp_head(a, coefs, ints)[0].numpy(), N.mlp_forward(a, coefs, ints), atol=5e-3)
+
+
+def test_cell_bound_covers_either_contraction():
+    """The compiler may fuse either product of c = f c_prev + i g (commit history: it chose differently once the IEEE
+    path was compiled alone), and the test hook's instance may fuse differently from the kernel's.  With the f32 gate
+    values taken as exact inputs (no gate error to absorb anything), the cell's own rounding terms must cover float32
+    emulations of all three forms: fma on f c_prev (i g rounded), fma on i g (f c_prev rounded), both rounded."""
+    z, cp = D.cell_grid()
+    d = lambda v: v.double()   # noqa: E731
+    i, f, o, g = (fn(d(torch.from_numpy(v))).float() for fn, v in ((torch.sigmoid, z[0]), (torch.sigmoid, z[1]),
+                                                                    (torch.sigmoid, z[3]), (torch.tanh, z[2])))
+    c32 = torch.from_numpy(cp)
+    forms = {"fma f*c": (d(f) * d(c32) + d(i * g)).float(), "fma i*g": (d(f * c32) + d(i) * d(g)).float(),
+             "rounded": f * c32 + i * g}
+    ig = d(i) * d(g)
+    zero = torch.zeros_like(ig)
+    c_ref, ec = D._cell_update(ig, D.U24 * ig.abs() + D.TINY, d(f), zero, d(c32), zero, True)
+    h_ref, eh = D._cell_out(c_ref, ec, d(o), zero, "exact", True)
+    worst = 0.0
+    for name, c in forms.items():
+        h = (d(o) * torch.tanh(d(c))).float()   # the tanh exact, one rounding of the product
+        rc = float(((d(c) - c_ref).abs() / ec).max())
+        rh = float(((d(h) - h_ref).abs() / eh).max())
+        assert rc <= 1 and rh <= 1, (name, rc, rh)
+        worst = max(worst, rc)
+    assert worst > 0.5   # the rounding terms are needed: the check is not slack

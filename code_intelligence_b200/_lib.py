@@ -39,6 +39,7 @@ PROTOTYPES = {
                                           C.c_void_p]),
     "ie_encoder_launch_count": (C.c_int64, [C.c_void_p]),
     "ie_encoder_max_batch": (C.c_int32, [C.c_void_p]),
+    "ie_debug_workspace_bytes": (C.c_int64, [C.c_void_p]),
     "ie_encoder_check_errors": (C.c_int, [C.c_void_p]),
     "ie_encoder_last_phase_ms": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     "ie_encoder_last_phase_mhz": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),

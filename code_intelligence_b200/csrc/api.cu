@@ -131,8 +131,7 @@ struct ie_encoder {
   int trace_layer = -1;
   int trace_T = 0, trace_ctas = 0;
   long long y_ld = 0;
-  long long ws_tokens = 0;  // largest b_pad*T the workspace was grown for
-  int small_calls = 0;      // consecutive calls far below ws_tokens (workspace is released after a few)
+  int small_calls = 0;      // consecutive calls far below the buffers that grow with T (workspace released after a few)
   cudaStream_t own_stream = nullptr;
   cudaStream_t last_stream = nullptr;
   cudaEvent_t done_ev = nullptr;  // end of the last call: a call on another stream waits for it (shared workspace)
@@ -235,19 +234,30 @@ long long max_out_pad(const ie_encoder* h) {
 void release_workspace(ie_encoder* h) {
   DevBuf* bufs[] = {&h->ids, &h->x0, &h->y[0], &h->y[1], &h->gx, &h->raw, &h->step_done, &h->tok};
   for (DevBuf* b : bufs) b->release();
-  h->ws_tokens = 0;
   h->small_calls = 0;
 }
 
+// bytes held by the buffers that grow with T (the token ids, their time-major copy and the raw states)
+long long t_bytes(const ie_encoder* h) {
+  return static_cast<long long>(h->ids.cap + h->tok.cap + h->raw.cap);
+}
+
 // The time dimension is processed in chunks of chunk_T steps (time-major: every layer runs a chunk before the next
-// chunk starts; c and h are carried per layer), so everything but the token ids is bounded by chunk_T * b_pad rows.
-int ensure_workspace(ie_encoder* h, int b_pad, int T, int chunk_T, bool want_raw, bool need_x0, bool need_tok) {
+// chunk starts; c and h are carried per layer), so everything but the token ids, their time-major copy and the raw
+// states is bounded by chunk_T * b_pad rows.  raw_ld > 0: the f32 states of one layer of out_pad raw_ld for the B valid
+// rows.  *t_need receives the bytes this call needs of the buffers that grow with T.
+int ensure_workspace(ie_encoder* h, int B, int b_pad, int T, int chunk_T, long long raw_ld, bool need_x0, bool need_tok,
+                     long long* t_need) {
   const ie_config& c = h->cfg;
   const long long mop = max_out_pad(h);
   const long long rows = static_cast<long long>(T) * b_pad;
   const long long crow = static_cast<long long>(chunk_T) * b_pad;
   const int ring_mul = h->segs > 1 ? 2 : 1;
-  CK(h->ids.reserve(static_cast<size_t>(h->max_batch) * T * sizeof(int64_t)));
+  const size_t ids_bytes = static_cast<size_t>(h->max_batch) * T * sizeof(int64_t);
+  const size_t raw_bytes = static_cast<size_t>(B) * T * raw_ld * sizeof(float);
+  const size_t tok_bytes = need_tok ? static_cast<size_t>(rows) * sizeof(int) : 0;
+  *t_need = static_cast<long long>(ids_bytes + raw_bytes + tok_bytes);
+  CK(h->ids.reserve(ids_bytes));
   CK(h->len_in.reserve(h->max_batch * sizeof(int)));
   CK(h->lengths.reserve(h->max_batch * sizeof(int)));
   CK(h->err.reserve(kErrWords * sizeof(int), true));
@@ -266,10 +276,9 @@ int ensure_workspace(ie_encoder* h, int b_pad, int T, int chunk_T, bool want_raw
   CK(h->pool_max.reserve(pb));
   CK(h->pool_last.reserve(pb));
   CK(h->out.reserve(static_cast<size_t>(h->max_batch) * 3 * c.emb_sz * sizeof(float)));
-  if (want_raw) CK(h->raw.reserve(static_cast<size_t>(b_pad) * T * mop * sizeof(float)));
+  if (raw_bytes) CK(h->raw.reserve(raw_bytes));
   CK(h->step_done.reserve(static_cast<size_t>(chunk_T) * ie::kMaxBatches * sizeof(unsigned)));
-  if (need_tok) CK(h->tok.reserve(static_cast<size_t>(rows) * sizeof(int)));
-  h->ws_tokens = std::max(h->ws_tokens, crow);
+  if (need_tok) CK(h->tok.reserve(tok_bytes));
   return IE_OK;
 }
 
@@ -381,7 +390,9 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
   if (h->chunk_t > 0) chunk_T = h->chunk_t;
   chunk_T = std::min<long long>(chunk_T, T);
   const bool proj = proj_usable(h);
-  int rc = ensure_workspace(h, b_pad, T, static_cast<int>(chunk_T), raw_out != nullptr, !proj, proj);
+  const long long raw_ld = raw_out != nullptr ? h->layers[raw_layer].out_pad : 0;
+  long long t_need = 0;
+  int rc = ensure_workspace(h, B, b_pad, T, static_cast<int>(chunk_T), raw_ld, !proj, proj, &t_need);
   if (rc != IE_OK) return rc;
   if (h->done_ev == nullptr) CK(cudaEventCreateWithFlags(&h->done_ev, cudaEventDisableTiming));
   // one workspace per handle: a call on another stream first waits for the previous call
@@ -497,7 +508,7 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
       q.abort_flag = h->err.as<unsigned>() + 1; q.spin_limit = h->spin_limit;
       q.T = Tc; q.t0 = static_cast<int>(t0); q.T_total = T; q.ng = ng;
       q.u = L.u; q.n_cta = L.n_cta; q.out_pad = L.out_pad; q.kh_pad = L.kh_pad;
-      q.ldy = h->y_ld; q.raw_ld = L.out_pad;
+      q.ldy = h->y_ld; q.raw_ld = L.out_pad; q.raw_rows = B;
       q.gate_mode = h->gate_mode; q.gx_bf16 = h->gx_bf16; q.segs = h->segs;
       q.num_sms = h->num_sms; q.check_only = 0; q.cooperative = h->cooperative; q.fault = h->fault;
       q.diag = h->diag.as<long long>() + 8 * l;
@@ -538,8 +549,6 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
       cur ^= 1;
     }
   }
-  const long long rows = static_cast<long long>(T) * b_pad;
-
   const Layer& LL = h->layers.back();
   if (pooled) {
     float* out_dev = dev ? out : h->out.as<float>();
@@ -551,7 +560,7 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
       CK(cudaMemcpyAsync(out, out_dev, static_cast<size_t>(B) * 3 * c.emb_sz * sizeof(float), cudaMemcpyDeviceToHost, s));
   }
   if (raw_out != nullptr) {
-    // raw workspace is [b_pad, T, out_pad] of the requested layer; compact to [B, T, out]
+    // raw workspace is [B, T, out_pad] of the requested layer; compact to [B, T, out]
     const Layer& LR = h->layers[raw_layer];
     CK(cudaMemcpy2DAsync(raw_out, static_cast<size_t>(LR.out) * sizeof(float), h->raw.p,
                          static_cast<size_t>(LR.out_pad) * sizeof(float), static_cast<size_t>(LR.out) * sizeof(float),
@@ -560,8 +569,11 @@ int run_encoder(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int B
   CK(cudaEventRecord(h->done_ev, s));
   h->has_done = true;
   h->last_stream = s;
-  // a handle that once served a very long sequence does not keep tens of GB for ever
-  if (h->ws_tokens > (1ll << 21) && std::min<long long>(rows, chunk_T * b_pad) * 8 < h->ws_tokens) {
+  // a handle that once served a very long sequence does not keep its T-sized buffers -- nor the time-chunk buffers a
+  // single long issue grows to 2^20 rows -- for ever: after four consecutive calls that need under 1/8 of the bytes
+  // held by the buffers that grow with T (and those hold over 64 MB) the workspace is released; the next call grows it
+  // to its own size.  Calls of one shape never trigger it, nor do the short calls that follow bulk encodes at T <= 4096.
+  if (t_bytes(h) > (64ll << 20) && t_need * 8 < t_bytes(h)) {
     if (++h->small_calls >= 4) {
       CK(cudaStreamSynchronize(s));
       release_workspace(h);
@@ -758,6 +770,17 @@ int ie_encoder_check_errors(ie_encoder* h) {
 int64_t ie_encoder_launch_count(const ie_encoder* h) { return h ? h->launches : 0; }
 
 int32_t ie_encoder_max_batch(const ie_encoder* h) { return h ? h->max_batch : IE_MAX_BATCH; }
+
+int64_t ie_debug_workspace_bytes(const ie_encoder* h) {
+  if (h == nullptr) return fail(IE_ERR_INVALID, "null handle");
+  std::lock_guard<std::mutex> lk(const_cast<ie_encoder*>(h)->mu);
+  const DevBuf* bufs[] = {&h->ids, &h->len_in, &h->lengths, &h->x0, &h->y[0], &h->y[1], &h->hcarry, &h->gx, &h->c,
+                          &h->pool_sum, &h->pool_max, &h->pool_last, &h->out, &h->raw, &h->err, &h->step_done,
+                          &h->diag, &h->trace, &h->tok};
+  int64_t n = 0;
+  for (const DevBuf* b : bufs) n += static_cast<int64_t>(b->cap);
+  return n;
+}
 
 // debug: request a per-item timeline of `layer` in the persistent kernel on the next encode (layer < 0: off);
 // with out != NULL copy the last recorded timeline [ctas][items][12] and return ctas*items

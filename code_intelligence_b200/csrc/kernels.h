@@ -68,7 +68,8 @@ struct LstmLayerArgs {
   const int* tok;          // optional time-major token ids of the whole call (per-token input-projection table)
   float* c;                // [b_pad, out_pad] cell state
   __nv_bfloat16* y;        // ring (slot 0 = h before the chunk (zeros at t0 = 0); slot t+1 = h_t, t chunk-local)
-  float* raw;              // optional [b_pad, T_total, raw_ld] f32 copy of h (get_raw_features)
+  float* raw;              // optional [raw_rows, T_total, raw_ld] f32 copy of h (get_raw_features)
+  int raw_rows;            // rows of raw: the call's valid rows B (padding rows of the batch are not stored)
   float* pool_sum;         // optional [b_pad, out_pad] (last layer only; formats: lstm_common.cuh)
   float* pool_max;
   float* pool_last;

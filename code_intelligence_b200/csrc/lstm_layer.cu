@@ -84,7 +84,7 @@ struct KArgs {
   const float* bias;     // FUSE: b_ih + b_hh, permuted, in fragment order (takes the place of Gx)
   float* cstate;         // [b_pad, out_pad]
   __nv_bfloat16* y;      // ring [(T+1)*b_pad, ldy] of this time chunk: slot 0 = h before the chunk, slot t+1 = h_t
-  float* raw;            // optional [b_pad, T_total, raw_ld]
+  float* raw;            // optional [raw_rows, T_total, raw_ld]: rows brow < raw_rows only
   float* pool_sum;       // optional (last layer)
   float* pool_max;
   float* pool_last;
@@ -95,7 +95,7 @@ struct KArgs {
   long long ldy, raw_ld;
   long long* trace;
   long long* diag;
-  int T, t_begin, t0, T_total, ng, tiles, out_pad, nkb, segs, kh_pad, trace_items, fault;
+  int T, t_begin, t0, T_total, ng, tiles, out_pad, nkb, segs, kh_pad, trace_items, fault, raw_rows;
   int pre_nkb;           // FUSE: k-blocks of the input projection that precede the recurrent ones in every item
 };
 
@@ -407,7 +407,7 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
           const float4 h4 = make_float4(hn[0], hn[1], hn[2], hn[3]);
           __stcg(reinterpret_cast<float4*>(cp + 16 * s), make_float4(cn[0], cn[1], cn[2], cn[3]));
           store_h4(yrow + 16 * s, h4, lo_off);
-          if (a.raw != nullptr)
+          if (a.raw != nullptr && brow < a.raw_rows)
             *reinterpret_cast<float4*>(a.raw + (static_cast<long long>(brow) * a.T_total + tg) * a.raw_ld + unit0 + 16 * s) = h4;
           if constexpr (POOL)
             pool_accumulate4(a.pool_sum, a.pool_max, a.pool_last, po + 16 * s, h4, tg, len, FUSE ? &mv[hr][s] : nullptr);
@@ -499,6 +499,7 @@ cudaError_t launch_layer_t(const LstmLayerArgs& a, int ctas, int tiles, cudaStre
   }
   KArgs k{};
   k.gx = a.gx; k.tok = a.tok; k.bias = a.bias; k.pre_nkb = FUSE ? a.pre_nkb : 0; k.cstate = a.c; k.y = a.y; k.raw = a.raw;
+  k.raw_rows = a.raw_rows;
   k.pool_sum = a.pool_sum; k.pool_max = a.pool_max; k.pool_last = a.pool_last; k.lengths = a.lengths;
   k.step_done = a.single_step ? nullptr : a.step_done; k.abort_flag = a.abort_flag;
   k.spin_limit = a.spin_limit > 0 ? a.spin_limit : kSpinLimitDefault;

@@ -187,6 +187,13 @@ class IssueEncoder:
         check(self._lib.ie_debug_layer_states(self._h, layer, ids.ctypes.data, B, T, out.ctypes.data, 0, None))
         return out
 
+    def _debug_workspace_bytes(self) -> int:
+        """Test hook ``ie_debug_workspace_bytes``: bytes of device workspace the handle holds now."""
+        n = int(self._lib.ie_debug_workspace_bytes(self._h))
+        if n < 0:
+            check(n)
+        return n
+
     @property
     def max_batch(self) -> int:
         """Rows one C-ABI encode call takes: 256 x batches per launch (1280 by default, IE_BATCHES=n changes it)."""

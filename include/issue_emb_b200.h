@@ -98,12 +98,17 @@ int ie_encoder_load_layer(ie_encoder* h, int32_t layer, const float* w_ih, const
  *   out     [B, 3*emb_sz] f32 = [mean | max | last] over the first lengths[b] steps of the last layer's hidden
  *           states, zero initial state (encoder.reset(), inference.py:56)
  * 1 <= B <= ie_encoder_max_batch(h).  T is bounded only by the workspace cap B_pad*T <= 2^27 tokens (IE_ERR_OOM
- * beyond; B_pad = B rounded up to 256): the time dimension is processed in chunks, so a single 16k-token issue is
- * fine. */
+ * beyond; B_pad = B rounded up to 256): the time dimension is processed in chunks of 2^20 / B_pad steps (half that
+ * with f32 input projections), so the device workspace stays under about 31 GB at the deployed shape whatever T is,
+ * and a single 16k-token issue is fine.  A handle keeps its workspace between calls; after four consecutive calls
+ * that need under 1/8 of the bytes held by the buffers that grow with T (over 64 MB of them), it is released. */
 int ie_encoder_encode(ie_encoder* h, const int64_t* ids, const int32_t* lengths, int32_t B, int32_t T, float* out,
                       int32_t flags, void* stream);
 
-/* InferenceWrapper.get_raw_features (inference.py:59-68): the last layer's hidden states, raw [B, T, emb_sz] f32. */
+/* InferenceWrapper.get_raw_features (inference.py:59-68): the last layer's hidden states, raw [B, T, emb_sz] f32.
+ * T is bounded as for ie_encoder_encode.  Device memory: the encode workspace (bounded by the time chunk) plus
+ * B * T * round_up(emb_sz, 64) * 4 bytes of f32 states for the B valid rows -- 41 MB for one 12 300-token issue at
+ * emb_sz = 800, 67 MB at 20 000 tokens. */
 int ie_encoder_raw_features(ie_encoder* h, const int64_t* ids, int32_t B, int32_t T, float* raw, int32_t flags,
                             void* stream);
 
@@ -113,6 +118,10 @@ int64_t ie_encoder_launch_count(const ie_encoder* h);
 /* Rows one ie_encoder_encode call accepts on this handle: 1280 = five 256-row batches per launch by default
  * (environment variable IE_BATCHES=n at create time, 1 <= n <= 12, changes that to 256 n). */
 int32_t ie_encoder_max_batch(const ie_encoder* h);
+
+/* Test hook: bytes of device workspace the handle holds now (the buffers its calls grow and reuse; weights, the
+ * embedding and the per-token table not included). */
+int64_t ie_debug_workspace_bytes(const ie_encoder* h);
 
 /* Device-side error state of the last call on this handle (waits for it to finish): IE_OK, IE_ERR_TOKEN (a token id
  * outside [0, vocab_sz) was remapped to 0), IE_ERR_INVALID (a length outside [1,T] was clamped; device-pointer mode

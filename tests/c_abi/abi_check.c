@@ -17,6 +17,7 @@ int main(void) {
   fn syms[] = {(fn)ie_version, (fn)ie_last_error, (fn)ie_encoder_create, (fn)ie_encoder_destroy,
                (fn)ie_encoder_load_embedding, (fn)ie_encoder_load_layer, (fn)ie_encoder_encode, (fn)ie_encoder_raw_features,
                (fn)ie_encoder_launch_count, (fn)ie_encoder_max_batch, (fn)ie_encoder_last_phase_ms, (fn)ie_debug_seq_trace,
+               (fn)ie_debug_workspace_bytes,
                (fn)ie_encoder_check_errors, (fn)ie_encoder_last_phase_mhz, (fn)ie_mlp_create, (fn)ie_mlp_load_layer, (fn)ie_mlp_predict_proba,
                (fn)ie_mlp_destroy, (fn)ie_pr_thresholds, (fn)ie_debug_gemm, (fn)ie_debug_gemm_ex,
                (fn)ie_debug_layer_states, (fn)ie_debug_gates};

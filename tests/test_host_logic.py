@@ -348,7 +348,7 @@ def test_c_abi_from_plain_c(tmp_path):
                     "-l:" + os.path.basename(_lib.LIB_PATH), "-Wl,-rpath," + libdir], check=True)
     r = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stdout + r.stderr
-    assert "version=200 symbols=23" in r.stdout, r.stdout
+    assert "version=200 symbols=24" in r.stdout, r.stdout
 
 
 def test_spacy_like_tokenizer_never_loses_characters():

@@ -67,6 +67,19 @@ PROTOTYPES = {
                                 C.c_void_p]),
     "ie_knn_check_errors": (C.c_int, [C.c_void_p]),
     "ie_debug_knn_shortlist": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "ie_mlp_train_create": (C.c_int, [C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_void_p)]),
+    "ie_mlp_train_destroy": (None, [C.c_void_p]),
+    "ie_mlp_train_set_layer": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "ie_mlp_train_get_layer": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "ie_mlp_train_set_data": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64]),
+    "ie_mlp_train_epoch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_double, C.c_double,
+                                     C.c_double, C.c_double, C.c_void_p]),
+    "ie_mlp_train_validation_proba": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "ie_mlp_train_snapshot": (C.c_int, [C.c_void_p, C.c_int32]),
+    "ie_mlp_train_launch_count": (C.c_int64, [C.c_void_p]),
+    "ie_mlp_train_last_epoch_ms": (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
+    "ie_debug_mlp_train_step": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_int64, C.POINTER(C.c_double)]),
 }
 
 _lib = None

@@ -158,4 +158,48 @@ cudaError_t launch_knn_merge_rerank(const uint2* cand, const int* cnt, int rows,
                                     const float* X, int D, int cosine, int k, float* out_dist, int64_t* out_idx,
                                     float* dbg_score, int64_t* dbg_idx, cudaStream_t stream);
 
+// ---- label-MLP training step (mlp_train.cu) -------------------------------------------------------------------------
+// src [rows, cols] f32 (row r read from src row rowidx[r] when rowidx is set; zeroed where mask [rows, ld_mask] is 0),
+// optionally copied to out_f32, stored as split-bf16 operands with exact zeros outside [rows, cols]:
+//   rm [rm_rows, ld_rm]: row r = [hi(rm_kpad) | lo(rm_kpad)]   (the A operand of the next product)
+//   tr [tr_rows, ld_tr]: row c = [hi(tr_kpad) | lo(tr_kpad)] of column c  (transposed: K = rows, for a weight gradient)
+struct SplitStoreArgs {
+  const float* src;
+  long long ld_src;
+  const int* rowidx;
+  int rows, cols;
+  const float* mask;
+  long long ld_mask;
+  float* out_f32;
+  long long ld_f32;
+  __nv_bfloat16* rm;
+  long long ld_rm;
+  int rm_rows, rm_kpad;
+  __nv_bfloat16* tr;
+  long long ld_tr;
+  int tr_rows, tr_kpad;
+};
+cudaError_t launch_split_store(const SplitStoreArgs& a, cudaStream_t stream);
+// rows b of z [b, ldz] (the last layer's pre-activation): p = sigmoid_acc(z); with Y (u8 [n, L], row rowidx[r]):
+// delta = p - y and row_loss[r] = sum over labels of log(clip(p)) or log(1 - clip(p)) (f64). p and delta share ldz.
+cudaError_t launch_mlp_output(const float* z, long long ldz, const uint8_t* Y, const int* rowidx, int b, int L, float* p,
+                              float* delta, double* row_loss, cudaStream_t stream);
+// gW [fan_in, fan_out] = f32((dw + f32(alpha) W) / b) with dw = a^T delta [fan_in, ld_dw]; gb [fan_out] = f32(sum_r delta / b)
+cudaError_t launch_mlp_grad(const float* dw, long long ld_dw, const float* W, int fan_in, int fan_out, const float* delta,
+                            long long ld_delta, int b, float alpha, float* gW, float* gb, cudaStream_t stream);
+// *out = -sum(row_loss[0..b)) / b + 0.5 alpha sum(sq_part) / b
+cudaError_t launch_mlp_loss(const double* row_loss, int b, const double* sq_part, int n_part, double alpha, double* out,
+                            cudaStream_t stream);
+constexpr int kAdamBlocks = 264;  // fixed grid: the sum |W|^2 partials are summed in the same order every step
+struct AdamArgs {
+  float *p, *m, *v;
+  const float* g;        // nullptr: no update, only the sum |W|^2 partials of p
+  long long n, n_coef;   // parameters, of which the first n_coef are coefficients
+  float beta1, one_m_beta1, beta2, one_m_beta2, eps;  // f32 roundings of the Python doubles
+  const double* lr;      // lr[step] = learning_rate_init sqrt(1 - beta2^t) / (1 - beta1^t)
+  int step;
+  double* sq_part;       // [kAdamBlocks]
+};
+cudaError_t launch_adam(const AdamArgs& a, cudaStream_t stream);
+
 }  // namespace ie

@@ -4,7 +4,8 @@
 ``predict_probabilities``, ``find_probability_thresholds``, ``grid_search``, ``save_model`` / ``load_model`` -- but
 ``predict_probabilities`` (mlp.py:56-63, sklearn ``MLPClassifier.predict_proba``) runs the fitted network's forward
 pass relu(relu(X W0 + b0) W1 + b1) ... -> sigmoid through the wgmma GEMM kernel behind ``ie_mlp_*``
-(include/issue_emb_b200.h).  Training-time methods stay on sklearn (out of scope, SURVEY.md section 2 row 5).
+(include/issue_emb_b200.h).  ``fit`` and ``grid_search`` train whatever estimator the wrapper holds: a plain sklearn
+``MLPClassifier`` fits on the host, ``mlp_train.DeviceMLPClassifier`` fits on the GPU (search it with ``n_jobs=1``).
 """
 from __future__ import annotations
 
@@ -143,7 +144,7 @@ class MLPWrapper:
         self.total_labels_count = None
 
     def fit(self, X, y):
-        """Train the classifier (sklearn on the CPU: training is out of scope of the GPU path)."""
+        """Train the classifier: on the host for sklearn's MLPClassifier, on the GPU for mlp_train.DeviceMLPClassifier."""
         self.clf.fit(X, y)
         self._head = None
 
@@ -161,7 +162,8 @@ class MLPWrapper:
         """mlp.py:65-98: hold out ``test_size`` of the data (random_state 1234), fit on the rest, and for every label keep
         the probability threshold with the highest precision among the points of its precision-recall curve that meet
         both ``precision_threshold`` and ``recall_threshold`` (first such point on ties; ``None`` when no point
-        qualifies, which makes the label unpredictable, repo_specific_model.py:138-141).  ``fit`` stays on sklearn; the
+        qualifies, which makes the label unpredictable, repo_specific_model.py:138-141).  ``fit`` trains the wrapped
+        estimator (on the GPU for mlp_train.DeviceMLPClassifier); the
         hold-out ``predict_proba`` and the per-label curve search run on the GPU (``ie_pr_thresholds``: sort + prefix sum +
         argmax per label in one kernel); hold-out sets above 16384 rows use sklearn's curve on the host."""
         from sklearn.model_selection import train_test_split

@@ -241,6 +241,44 @@ int ie_knn_check_errors(ie_knn* h);
  * index: score [nq, k + 32] f32 and idx [nq, k + 32] int64 (-1 / -inf past the rows stored). */
 int ie_debug_knn_shortlist(ie_knn* h, const float* Q, int32_t nq, int32_t k, float* score, int64_t* idx);
 
+/* Label-MLP trainer.  Replaces the step loop of sklearn MLPClassifier.fit(solver='adam', activation='relu') on a
+ * logistic (multilabel / binary) output, as MLPWrapper.fit calls it (py/label_microservice/mlp.py:45-54); the host
+ * driver (code_intelligence_b200/mlp_train.py) keeps every decision sklearn makes -- initialisation, validation split,
+ * row orders, stopping -- and calls these once per epoch.  Host pointers only; every call returns when its work is done.
+ *   dims [n_layers + 1] = {D_in, hidden..., n_labels}, n_layers >= 2 (at least one hidden layer).
+ *   Parameters are f32 in sklearn's layout: coef_l [dims[l], dims[l+1]] (coefs_[l]), intercept_l [dims[l+1]].
+ *   Every product is a split-bf16 GEMM (segs 3); the loss is float64; the Adam step is sklearn's AdamOptimizer on float32
+ *   arrays bit for bit (DESIGN.md section 9). */
+typedef struct ie_mlp_train ie_mlp_train;
+int ie_mlp_train_create(int32_t n_layers, const int32_t* dims, int32_t device, ie_mlp_train** out);
+void ie_mlp_train_destroy(ie_mlp_train* h);
+/* Set (and reset the Adam moments of every layer to zero, t = 0) / read one layer's current (best = 0) or snapshot
+ * (best = 1) parameters.  Non-finite values are refused. */
+int ie_mlp_train_set_layer(ie_mlp_train* h, int32_t layer, const float* coef, const float* intercept);
+int ie_mlp_train_get_layer(ie_mlp_train* h, int32_t layer, int32_t best, float* coef, float* intercept);
+/* Resident data: which 0 = training set X [n, D_in] f32 and Y [n, n_labels] u8 (0/1), which 1 = validation X (Y unused).
+ * A non-finite X value returns IE_ERR_INVALID. */
+int ie_mlp_train_set_data(ie_mlp_train* h, int32_t which, const float* X, const uint8_t* Y, int64_t n);
+/* One epoch: steps k = 0 .. ceil(n / batch_size) - 1 on training rows order[k*batch_size ...] (the last batch short),
+ * learning rate lr[k] = learning_rate_init sqrt(1 - beta_2^t) / (1 - beta_1^t) of the step's t; losses[k] receives each
+ * step's batch loss (log loss + 0.5 alpha sum|W|^2 / b).  The steps are enqueued without host synchronisation. */
+int ie_mlp_train_epoch(ie_mlp_train* h, const int32_t* order, int64_t n, int32_t batch_size, const double* lr,
+                       double alpha, double beta_1, double beta_2, double epsilon, double* losses);
+/* Probabilities [n_val, n_labels] f32 of the validation set under the current parameters. */
+int ie_mlp_train_validation_proba(ie_mlp_train* h, float* probs);
+/* restore 0: snapshot the current parameters as the best; 1: make the snapshot current again. */
+int ie_mlp_train_snapshot(ie_mlp_train* h, int32_t restore);
+/* Kernels launched by this handle so far / device time (CUDA events) of the last ie_mlp_train_epoch. */
+int64_t ie_mlp_train_launch_count(const ie_mlp_train* h);
+int ie_mlp_train_last_epoch_ms(ie_mlp_train* h, float* ms);
+/* Debug / test hook.  mode 0: one forward + backward pass on training rows rows[b] with consts[0] = alpha, parameters
+ * unchanged: out = a_1 .. a_{n_layers-1} (hidden activations), p (probabilities), delta_0 .. delta_{n_layers-1} (each
+ * [b, width] f32, delta_l = dLoss/dz of layer l's output, sklearn's deltas[l]), then the gradients in sklearn's packing
+ * (every coef, then every intercept); *loss = the batch loss.  mode 1: one optimizer step with the given gradients
+ * (sklearn's packing) and consts = {lr_t, beta_1, beta_2, epsilon}: out = parameters, m, v, each in sklearn's packing. */
+int ie_debug_mlp_train_step(ie_mlp_train* h, int32_t mode, const int32_t* rows, int32_t b, const double* consts,
+                            const float* grads, float* out, int64_t cap, double* loss);
+
 #ifdef __cplusplus
 }
 #endif

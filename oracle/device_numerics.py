@@ -472,14 +472,18 @@ def pool(h, lengths, mutant: str | None = None) -> np.ndarray:
 def gemm_interval(a, b, bias, act: int, out_type: str, segs: int, device=None):
     """Where each element of act(a b^T + bias), computed by the library's GEMM and stored as out_type, must lie.
     segs 1: the f64 product of the bf16-rounded operands +- the accumulation bound; segs 3: the f64 product of the
-    ORIGINAL f32 operands +- SPLIT_REL * sum|a b| (split-bf16 drops lo*lo and the residual of x - hi - lo) +- the
-    accumulation bound of the three-pass chain.
+    ORIGINAL f32 operands +- what split-bf16 drops (lo*lo and the residuals of x - hi - lo), taken exactly as the
+    difference from the f64 sum of the three passes' products, +- the accumulation bound of the three-pass chain.
+    SPLIT_REL * sum|a b| is no bound on the dropped terms: one dominant product can lose nearly 3 * 2^-16 of itself,
+    and operands whose lo part falls below bf16's normal range (|x| < 2^-118) lose more.
     Returns (lo, hi, ref) float64 torch tensors [M, N]; ref is the unrounded value."""
     a, b = _t(a, device), _t(b, device)
     _, sa, ss = chain(passes(operands(a, segs), operands(b, segs), segs))
     if segs == 3:
         z = a @ b.T
-        eps = SPLIT_REL * (a.abs() @ b.abs().T) + acc_err(ss, sa)
+        zs, _ = products(operands(a, 3), operands(b, 3), 3)
+        # the two f64 sums carry at most K * 2^-53 of sum|a b| each
+        eps = (z - zs).abs() + a.shape[1] * 2.0 ** -51 * sa + acc_err(ss, sa)
     else:
         z, _ = products(operands(a, 1), operands(b, 1), 1)
         eps = acc_err(ss, sa)

@@ -9,12 +9,18 @@ sklearn's random draws and decisions.
 ``adam_f32`` is the float32 Adam step the device implements (csrc/mlp_train.cu adam_kernel), written with explicit
 roundings instead of NumPy's promotion rules: each f32 product and sum rounded on its own, the learning rate and the
 update in float64, the parameter rounded once from f64(p) + update.
+
+``check_step`` checks one training step of the device (``DeviceSteps.debug_step``) stage by stage, each stage fed the
+device's own f32 inputs, against the bounds of DESIGN.md section 2 "Bounds of the training step".
 """
 from __future__ import annotations
 
 import numpy as np
+import torch
 from scipy.special import expit, xlogy
 from sklearn.utils import gen_batches
+
+from . import device_numerics as DN
 
 
 def binary_log_loss(y_true, y_prob):
@@ -131,3 +137,62 @@ def adam_f32(params, grads, ms, vs, lr_t, beta_1=0.9, beta_2=0.999, epsilon=1e-8
         out_m.append(m.astype(f32))
         out_v.append(v.astype(f32))
     return out_p, out_m, out_v
+
+
+def _check_in(name, dev, lo, hi, ref, stats):
+    """dev inside [lo, hi] elementwise; stats[name] = max |dev - ref| / eps with eps the wider side of the interval."""
+    dev = torch.as_tensor(np.asarray(dev, dtype=np.float64), device=lo.device)
+    ok = (dev >= lo) & (dev <= hi)
+    eps = torch.maximum(hi - ref, ref - lo).clamp_min(1e-30)
+    stats[name] = float(((dev - ref).abs() / eps).max())
+    assert bool(ok.all()), (name, int((~ok).sum()), stats[name])
+
+
+def check_step(out, X, Y, rows, coefs, intercepts, alpha, device=None) -> dict:
+    """Every stage of one device step on rows `rows` of (X, Y) at parameters (coefs, intercepts), fed the device's own
+    f32 inputs from `out` (``DeviceSteps.debug_step``), inside its bound: hidden activations and p (``gemm_interval``,
+    segs 3), the output delta p - y exactly, the masked deltas (exactly 0 where the device's activation is 0), the coef
+    gradients through the monotone f32 add and divide, the intercept gradients and the f64 loss.  An AssertionError
+    whose first item names the stage on the first one outside; otherwise {stage: max |dev - ref| / eps}.  `device` is
+    where the float64 references are computed (None: the CPU)."""
+    f32 = np.float32
+    rows = np.asarray(rows)
+    b = len(rows)
+    stats = {}
+    x = np.asarray(X[rows], dtype=f32)
+    nl = len(coefs)
+    ins = [x] + list(out["acts"])
+    for l in range(nl - 1):
+        lo, hi, ref = DN.gemm_interval(ins[l], coefs[l].T, intercepts[l], 1, "f32", 3, device)
+        _check_in(f"a{l + 1}", out["acts"][l], lo, hi, ref, stats)
+    lo, hi, ref = DN.gemm_interval(ins[-1], coefs[-1].T, intercepts[-1], 2, "f32", 3, device)
+    _check_in("p", out["p"], lo, hi, ref, stats)
+    y = np.asarray(Y[rows]).astype(f32)
+    assert np.array_equal(out["deltas"][-1], (out["p"] - y).astype(f32)), (f"delta{nl - 1}",)
+    for l in range(nl - 1, 0, -1):
+        lo, hi, ref = DN.gemm_interval(out["deltas"][l], coefs[l], None, 0, "f32", 3, device)
+        mask = torch.as_tensor(out["acts"][l - 1] != 0, device=lo.device)
+        zero = torch.zeros_like(lo)
+        lo, hi, ref = torch.where(mask, lo, zero), torch.where(mask, hi, zero), torch.where(mask, ref, zero)
+        _check_in(f"delta{l - 1}", out["deltas"][l - 1], lo, hi, ref, stats)
+    for l in range(nl):
+        lo, hi, ref = DN.gemm_interval(ins[l].T, out["deltas"][l].T, None, 0, "f32", 3, device)
+        aw = (f32(alpha) * coefs[l]).astype(f32)
+        fin = [torch.as_tensor((((t.cpu().numpy().astype(f32) + aw).astype(f32)) / f32(b)).astype(f32)
+                               .astype(np.float64), device=lo.device) for t in (lo, hi)]
+        _check_in(f"coef_grad{l}", out["coef_grads"][l], fin[0], fin[1],
+                  (ref + torch.as_tensor(aw.astype(np.float64), device=lo.device)) / b, stats)
+        dl = out["deltas"][l].astype(np.float64)
+        ref_b = dl.sum(0) / b
+        eps_b = 2.0 ** -24 * np.abs(ref_b) + b * 2.0 ** -53 * np.abs(dl).sum(0) / b + DN.TINY
+        err = np.abs(out["intercept_grads"][l] - ref_b)
+        stats[f"intercept_grad{l}"] = float((err / eps_b).max())
+        assert (err <= eps_b).all(), (f"intercept_grad{l}", stats)
+    pc = np.clip(out["p"].astype(np.float64), 2.0 ** -23, 1 - 2.0 ** -23)
+    terms = np.where(np.asarray(Y[rows]) != 0, np.log(pc), np.log1p(-pc))
+    reg = 0.5 * alpha * sum(float((c.astype(np.float64) ** 2).sum()) for c in coefs) / b
+    ref_loss = -terms.sum() / b + reg
+    eps_loss = 1e-13 * (np.abs(terms).sum() / b + reg)
+    stats["loss"] = abs(out["loss"] - ref_loss) / eps_loss
+    assert abs(out["loss"] - ref_loss) <= eps_loss, ("loss", stats)
+    return stats

@@ -8,10 +8,8 @@ import warnings
 
 import numpy as np
 import pytest
-import torch
 
 from code_intelligence_b200.mlp_train import DeviceMLPClassifier, DeviceSteps
-from oracle import device_numerics as DN
 from oracle import mlp_train_ref as R
 
 pytestmark = pytest.mark.gpu
@@ -74,74 +72,69 @@ SHAPES = {   # (D, hidden, L, b)
     "binary_L1": (80, (40,), 1, 90),
     "L257": (120, (260,), 257, 130),
 }
+# edge cases on a shape of SHAPES: alpha; the last layer's intercepts (saturated outputs: +40 gives p = 1.0f exactly,
+# -40 a p far below the loss's clip, about -88 a zero from __fdividef's denominator above 2^126, -100 a zero from an
+# infinite one); a dead first hidden layer (every relu output 0); constant label columns; X scaled by a power of two
+EDGES = {
+    "alpha0": ("b65", dict(alpha=0.0)),
+    "alpha1e-4_production": ("production", dict(alpha=1e-4)),
+    "alpha10": ("b65", dict(alpha=10.0)),
+    "out_bias+40": ("b65", dict(out_bias=40.0)),
+    "out_bias-40": ("b65", dict(out_bias=-40.0)),
+    "out_bias-88": ("b65", dict(out_bias=-88.0)),
+    "out_bias-100": ("b65", dict(out_bias=-100.0)),
+    "dead_hidden": ("b65", dict(dead=True)),
+    "constant_labels": ("short_last_batch", dict(constant_labels=True)),
+    "x_scale_2^20": ("b65", dict(x_scale=2.0 ** 20)),
+    "x_scale_2^-40": ("b65", dict(x_scale=2.0 ** -40)),
+}
 
 
-def _check_in(name, dev, lo, hi, ref, stats):
-    dev = torch.as_tensor(np.asarray(dev, dtype=np.float64))
-    ok = (dev >= lo) & (dev <= hi)
-    eps = torch.maximum(hi - ref, ref - lo).clamp_min(1e-30)
-    stats[name] = float(((dev - ref).abs() / eps).max())
-    assert bool(ok.all()), (name, int((~ok).sum()), stats[name])
-
-
-@pytest.mark.parametrize("shape", list(SHAPES))
+@pytest.mark.parametrize("shape", list(SHAPES) + list(EDGES))
 def test_one_step_teacher_forced_per_stage(shape):
     """Each stage of one step, fed the device's own inputs, lies inside its bound (DESIGN.md section 9): activations,
     probabilities, output deltas (exact), masked deltas, coef and intercept gradients, the batch loss.  The edge shapes
-    put rows and columns of padding into every product: a padding row or column that contributed would leave a bound."""
-    D, hidden, L, b = SHAPES[shape]
+    put rows and columns of padding into every product: a padding row or column that contributed would leave a bound.
+    The edge cases reach the loss's clip with both label values, exact zeros through a dead layer, and inputs far from
+    unit scale."""
+    base, knobs = EDGES.get(shape, (shape, {}))
+    D, hidden, L, b = SHAPES[base]
     units = [D, *hidden, L]
     rng = np.random.default_rng(3)
     n = max(2 * b, 300)
-    X = rng.standard_normal((n, D)).astype(np.float32)
+    X = rng.standard_normal((n, D)).astype(np.float32) * np.float32(knobs.get("x_scale", 1.0))
     Y = (rng.random((n, L)) < 0.3).astype(np.uint8)
+    if knobs.get("constant_labels"):
+        Y[:, 0::3] = 0
+        Y[:, 1::3] = 1
     coefs, ints = _init(units, 4)
-    alpha = 1e-2
+    if "out_bias" in knobs:
+        ints[-1][:] = knobs["out_bias"]
+    if knobs.get("dead"):
+        ints[0][:] = -1e3
+    alpha = knobs.get("alpha", 1e-2)
     steps = DeviceSteps(units)
     steps.set_params(coefs, ints)
     steps.set_data(X, Y)
     rows = rng.choice(n, b, replace=False).astype(np.int32)
     out = steps.debug_step(rows, alpha)
     steps.close()
-    stats = {}
-    x = X[rows]
-    nl = len(coefs)
-    ins = [x] + out["acts"]
-    for l in range(nl - 1):
-        lo, hi, ref = DN.gemm_interval(ins[l], coefs[l].T, ints[l], 1, "f32", 3)
-        _check_in(f"a{l + 1}", out["acts"][l], lo, hi, ref, stats)
-    lo, hi, ref = DN.gemm_interval(ins[-1], coefs[-1].T, ints[-1], 2, "f32", 3)
-    _check_in("p", out["p"], lo, hi, ref, stats)
-    y = Y[rows].astype(np.float32)
-    assert np.array_equal(out["deltas"][-1], (out["p"] - y).astype(np.float32))
-    for l in range(nl - 1, 0, -1):
-        lo, hi, ref = DN.gemm_interval(out["deltas"][l], coefs[l], None, 0, "f32", 3)
-        mask = torch.as_tensor(out["acts"][l - 1] != 0)
-        zero = torch.zeros_like(lo)
-        lo, hi, ref = torch.where(mask, lo, zero), torch.where(mask, hi, zero), torch.where(mask, ref, zero)
-        _check_in(f"delta{l - 1}", out["deltas"][l - 1], lo, hi, ref, stats)
-    f32 = np.float32
-    for l in range(nl):
-        lo, hi, ref = DN.gemm_interval(ins[l].T, out["deltas"][l].T, None, 0, "f32", 3)
-        aw = (f32(alpha) * coefs[l]).astype(f32)
-        fin = [torch.as_tensor((((t.numpy().astype(f32) + aw).astype(f32)) / f32(b)).astype(f32).astype(np.float64))
-               for t in (lo, hi)]
-        _check_in(f"coef_grad{l}", out["coef_grads"][l], fin[0], fin[1],
-                  (ref + torch.as_tensor(aw.astype(np.float64))) / b, stats)
-        dl = out["deltas"][l].astype(np.float64)
-        ref_b = dl.sum(0) / b
-        eps_b = 2.0 ** -24 * np.abs(ref_b) + b * 2.0 ** -53 * np.abs(dl).sum(0) / b + DN.TINY
-        err = np.abs(out["intercept_grads"][l] - ref_b)
-        stats[f"intercept_grad{l}"] = float((err / eps_b).max())
-        assert (err <= eps_b).all(), (l, stats)
-    pc = np.clip(out["p"].astype(np.float64), 2.0 ** -23, 1 - 2.0 ** -23)
-    terms = np.where(Y[rows] != 0, np.log(pc), np.log1p(-pc))
-    reg = 0.5 * alpha * sum(float((c.astype(np.float64) ** 2).sum()) for c in coefs) / b
-    ref_loss = -terms.sum() / b + reg
-    eps_loss = 1e-13 * (np.abs(terms).sum() / b + reg)
-    stats["loss"] = abs(out["loss"] - ref_loss) / eps_loss
+    stats = R.check_step(out, X, Y, rows, coefs, ints, alpha)
     print(shape, {k: round(v, 3) for k, v in stats.items()})
-    assert abs(out["loss"] - ref_loss) <= eps_loss
+    f32 = np.float32
+    if "out_bias" in knobs:   # the clip is reached with both label values
+        pc = np.clip(out["p"], f32(2.0 ** -23), f32(1 - 2.0 ** -23))
+        clipped = pc != out["p"]
+        assert (clipped & (Y[rows] == 0)).any() and (clipped & (Y[rows] == 1)).any()
+        if knobs["out_bias"] == 40.0:
+            assert (out["p"] == 1.0).all()
+        if knobs["out_bias"] <= -88.0:
+            assert (out["p"] == 0.0).any()
+    if knobs.get("dead"):     # exact: a1 = 0, so delta0 = 0 and the first two coef gradients are f32(f32(alpha W) / b)
+        assert (out["acts"][0] == 0).all() and (out["deltas"][0] == 0).all() and (out["intercept_grads"][0] == 0).all()
+        for l in (0, 1):
+            want = ((f32(alpha) * coefs[l]).astype(f32) / f32(b)).astype(f32)
+            assert np.array_equal(out["coef_grads"][l].view(np.uint32), want.view(np.uint32)), l
 
 
 # ------------------------------------------------------------------------------------------------ decisions

@@ -192,3 +192,76 @@ def test_mlp_train_cu_built_for_sm_90a_reports_registers_and_spills():
     spills = [int(s) for s in re.findall(r"(\d+) bytes spill stores", text)]
     regs = [int(r) for r in re.findall(r"Used (\d+) registers", text)]
     assert len(regs) == 5 and max(regs) <= 64 and not any(spills)
+
+
+def _device_like_step(X, Y, rows, coefs, ints, alpha):
+    """One training step in float64 from the float32 inputs, rounded to f32 where the device rounds: every activation,
+    p, every delta (the masked ones on the f32 activation), the product a^T delta, the add of f32(alpha) W and the
+    division by b; the intercept gradient and the loss in f64 from those values, as DeviceSteps.debug_step returns it."""
+    f32, f64 = np.float32, np.float64
+    b, nl = len(rows), len(coefs)
+    a = [X[rows].astype(f32)]
+    for l in range(nl):
+        z = a[-1].astype(f64) @ coefs[l].astype(f64) + ints[l].astype(f64)
+        a.append((np.maximum(z, 0) if l < nl - 1 else 1.0 / (1.0 + np.exp(-z))).astype(f32))
+    p = a[-1]
+    d = [None] * nl
+    d[-1] = (p - Y[rows].astype(f32)).astype(f32)
+    for l in range(nl - 1, 0, -1):
+        d[l - 1] = np.where(a[l] != 0, (d[l].astype(f64) @ coefs[l].T.astype(f64)).astype(f32), f32(0))
+    cg = [(((a[l].T.astype(f64) @ d[l].astype(f64)).astype(f32) + (f32(alpha) * coefs[l]).astype(f32)).astype(f32)
+           / f32(b)).astype(f32) for l in range(nl)]
+    ig = [(d[l].astype(f64).sum(0) / b).astype(f32) for l in range(nl)]
+    pc = np.clip(p.astype(f64), 2.0 ** -23, 1 - 2.0 ** -23)
+    terms = np.where(Y[rows] != 0, np.log(pc), np.log1p(-pc))
+    loss = -terms.sum() / b + 0.5 * alpha * sum(float((c.astype(f64) ** 2).sum()) for c in coefs) / b
+    return {"acts": a[1:-1], "p": p, "deltas": d, "coef_grads": cg, "intercept_grads": ig, "loss": float(loss)}
+
+
+def _stage_failing(out, X, Y, rows, coefs, ints, alpha):
+    try:
+        R.check_step(out, X, Y, rows, coefs, ints, alpha)
+    except AssertionError as e:
+        return e.args[0][0]
+    return None
+
+
+@pytest.mark.parametrize("layer", [0, 2])
+def test_step_checker_accepts_a_device_like_step_and_rejects_stale_rows_and_unmasked_deltas(layer):
+    """oracle.mlp_train_ref.check_step is sharp enough for what it is meant to catch: it accepts a step rounded where
+    the device rounds, and rejects (at the right stage) the same step whose coef gradient of one layer also carries
+    28 rows of another batch (workspace rows of an earlier batch left in a short batch's K padding), and one whose
+    masked delta lets through a single element where the activation is 0."""
+    units = [40, 24, 16, 5]
+    rng = np.random.default_rng(17)
+    n, b, alpha = 300, 57, 1e-2
+    X = rng.standard_normal((n, units[0])).astype(np.float32)
+    Y = (rng.random((n, units[-1])) < 0.3).astype(np.uint8)
+    coefs, ints = [], []
+    for fi, fo in zip(units[:-1], units[1:]):
+        bound = np.sqrt(6.0 / (fi + fo))
+        coefs.append(rng.uniform(-bound, bound, (fi, fo)).astype(np.float32))
+        ints.append(rng.uniform(-bound, bound, fo).astype(np.float32))
+    order = rng.permutation(n).astype(np.int32)
+    rows, stale = order[:b], order[b:b + 28]
+    out = _device_like_step(X, Y, rows, coefs, ints, alpha)
+    stats = R.check_step(out, X, Y, rows, coefs, ints, alpha)
+    assert max(stats.values()) <= 1.0, stats
+
+    # 28 extra rows in layer `layer`'s product a^T delta, divided by the batch's own b
+    both = _device_like_step(X, Y, np.concatenate([rows, stale]), coefs, ints, alpha)
+    a_all = ([X[np.concatenate([rows, stale])]] + both["acts"])[layer].astype(np.float64)
+    d_all = both["deltas"][layer].astype(np.float64)
+    f32 = np.float32
+    dw = (a_all[:b].T @ d_all[:b] + a_all[b:].T @ d_all[b:]).astype(f32)
+    bad = dict(out, coef_grads=list(out["coef_grads"]))
+    bad["coef_grads"][layer] = ((dw + (f32(alpha) * coefs[layer]).astype(f32)).astype(f32) / f32(b)).astype(f32)
+    assert _stage_failing(bad, X, Y, rows, coefs, ints, alpha) == f"coef_grad{layer}"
+
+    # one delta not masked: an element where the f32 activation is 0 keeps its product value
+    l = 1 if layer == 0 else 0
+    unmasked = (out["deltas"][l + 1].astype(np.float64) @ coefs[l + 1].T.astype(np.float64)).astype(f32)
+    r, c = np.argwhere((out["acts"][l] == 0) & (unmasked != 0))[0]
+    bad = dict(out, deltas=[x.copy() for x in out["deltas"]])
+    bad["deltas"][l][r, c] = unmasked[r, c]
+    assert _stage_failing(bad, X, Y, rows, coefs, ints, alpha) == f"delta{l}"

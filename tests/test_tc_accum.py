@@ -128,6 +128,24 @@ def test_split_constants_on_coherent_f32_sums(K, factor):
     assert (err <= e_knn).all()
 
 
+def test_split_drop_of_one_dominant_product():
+    """Split-bf16 drops lo*lo and the residuals of x - hi - lo: on one product that reaches more than 2^-16 of |ab| (up
+    to nearly 3 * 2^-16), so SPLIT_REL * sum|ab| is no bound where one product dominates a sum (the training step's
+    K = 1 and sparse relu products met it on the H100), and for operands near 2^-126, whose lo part is a bf16 subnormal,
+    far more.  gemm_interval charges the dropped terms exactly, and the emulated device product lies inside it."""
+    r = np.random.default_rng(3)
+    for scale in (1.0, 2.0 ** -125):
+        a = (r.uniform(1, 2, (2048, 1)) * scale).astype(np.float32)
+        b = r.uniform(1, 2, (2048, 1)).astype(np.float32)
+        got = T.emulate(a, b, 3).astype(np.float64)
+        exact = a[:, 0].astype(np.float64) * b[:, 0]
+        rel = np.abs(got - exact) / (D.SPLIT_REL * exact)
+        assert rel.max() > (1.1 if scale == 1.0 else 100), rel.max()
+        lo, hi, _ = D.gemm_interval(a, b, None, 0, "f32", 3)
+        g = torch.from_numpy(got)
+        assert ((g >= lo.diagonal()) & (g <= hi.diagonal())).all()
+
+
 def test_acc_step_is_the_models_bound():
     assert D.ACC_STEP == T.acc_err_bound(1.0, 0.0) == K_REF.ACC_STEP
 

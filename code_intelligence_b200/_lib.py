@@ -80,6 +80,22 @@ PROTOTYPES = {
     "ie_mlp_train_last_epoch_ms": (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
     "ie_debug_mlp_train_step": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_int64, C.POINTER(C.c_double)]),
+    "ie_mlp_group_capacity": (C.c_int, [C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_double,
+                                        C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "ie_mlp_group_create": (C.c_int, [C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32,
+                                      C.POINTER(C.c_void_p)]),
+    "ie_mlp_group_destroy": (None, [C.c_void_p]),
+    "ie_mlp_group_set_data": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]),
+    "ie_mlp_group_set_layer": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "ie_mlp_group_get_layer": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "ie_mlp_group_set_hyper": (C.c_int, [C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_double]),
+    "ie_mlp_group_set_validation": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]),
+    "ie_mlp_group_epoch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p]),
+    "ie_mlp_group_validation_proba": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "ie_mlp_group_snapshot": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
+    "ie_mlp_group_launch_count": (C.c_int64, [C.c_void_p]),
+    "ie_mlp_group_last_epoch_ms": (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
 }
 
 _lib = None

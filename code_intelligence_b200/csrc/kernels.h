@@ -202,4 +202,87 @@ struct AdamArgs {
 };
 cudaError_t launch_adam(const AdamArgs& a, cudaStream_t stream);
 
+// ---- grouped label-MLP training (mlp_group.cu) ----------------------------------------------------------------------
+// Each launch runs the stage above for `count` models of one architecture: model j is slot slots[j] (device array),
+// its operands at base + slot * stride (strides in elements; 0 = shared by every model, as X and Y are).
+struct GroupSplitArgs {
+  SplitStoreArgs a;                                   // slot 0's operands
+  long long s_src, s_idx, s_mask, s_f32, s_rm, s_tr;
+  const int* slots;
+  int count;
+};
+cudaError_t launch_group_split_store(const GroupSplitArgs& g, cudaStream_t stream);
+struct GroupOutputArgs {   // launch_mlp_output per model; p and delta share z's pitch ldz and stride s_z
+  const float* z;
+  float *p, *delta;
+  long long ldz, s_z, s_p;
+  const uint8_t* Y;
+  const int* rowidx;
+  long long s_idx;
+  double* row_loss;
+  long long s_rl;
+  int b, L;
+  const int* slots;
+  int count;
+};
+cudaError_t launch_group_output(const GroupOutputArgs& g, cudaStream_t stream);
+struct GroupGradArgs {     // launch_mlp_grad per model; alpha[slot] (f64, rounded to f32 as the single step does)
+  const float* dw;
+  long long ld_dw, s_dw;
+  const float* W;          // and gW, gb: inside the parameter vectors, stride s_param
+  float *gW, *gb;
+  long long s_param;
+  const float* delta;
+  long long ld_delta, s_delta;
+  int fan_in, fan_out, b;
+  const double* alpha;
+  int coef_blocks;         // set by the launcher
+  const int* slots;
+  int count;
+};
+cudaError_t launch_group_grad(GroupGradArgs g, cudaStream_t stream);
+struct GroupLossArgs {     // launch_mlp_loss per model: out[slot * s_out] from row_loss and sq_part[slot][kAdamBlocks]
+  const double* row_loss;
+  long long s_rl;
+  const double* sq_part;
+  const double* alpha;
+  double* out;
+  long long s_out;
+  int b;
+  const int* slots;
+  int count;
+};
+cudaError_t launch_group_loss(const GroupLossArgs& g, cudaStream_t stream);
+struct GroupAdamArgs {     // launch_adam per model: consts[slot][5] = f32 beta1, 1 - beta1, beta2, 1 - beta2, eps
+  float *p, *m, *v;
+  const float* g;          // nullptr: only the sum |W|^2 partials
+  long long n, n_coef, s_param;
+  const float* consts;
+  const double* lr;        // lr[slot * s_lr + step]
+  long long s_lr;
+  int step;
+  double* sq_part;         // [slot][kAdamBlocks]
+  const int* slots;
+  int count;
+};
+cudaError_t launch_group_adam(const GroupAdamArgs& a, cudaStream_t stream);
+// D = act(A B^T + bias) for each model (segs = 3): A rows slot * a_rows + [0, m_pad), B rows slot * b_rows + [0, n_pad)
+// of stacked split-bf16 operands (a_rows % 128 == 0, b_rows % 256 == 0, zero rows past each model's extent), D and bias
+// at slot * s_d / s_bias; stored like launch_gemm_bf16's f32 output (rows < m_store, columns < n_store)
+struct GroupGemmArgs {
+  const __nv_bfloat16* a;
+  const __nv_bfloat16* b;
+  long long lda, ldb, a_rows, b_rows;
+  float* d;
+  long long ldd, s_d;
+  const float* bias;
+  long long s_bias;
+  int m_pad, n_pad, k_pad, m_store, n_store, relu;
+  int n_models;            // slots in the stacked operands
+  const int* slots;
+  int count;
+  int num_sms;
+};
+cudaError_t launch_group_gemm(const GroupGemmArgs& g, cudaStream_t stream);
+
 }  // namespace ie

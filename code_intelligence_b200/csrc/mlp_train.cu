@@ -10,6 +10,10 @@
 //   adam_kernel          sklearn AdamOptimizer on float32 arrays, bit for bit, plus per-block f64 partials of sum|W|^2
 //
 // Every reduction runs in a fixed order without atomics, so a fit is deterministic.
+//
+// mlp_group.cu repeats each of these kernels for many models at once, and api.cu's mg_* sequence repeats mt_forward /
+// mt_backward / mt_adam; a grouped fit is bit-identical to a single one only while each pair does the same arithmetic
+// over the same partition, so change both together (tests/test_gpu_mlp_grid_search.py checks the pairs bit for bit).
 #include <cuda_bf16.h>
 
 #include <algorithm>

@@ -189,7 +189,10 @@ class MLPWrapper:
                       'alpha': [.001, .01, .1, 1, 10],
                       'learning_rate': ['constant', 'adaptive'],
                       'learning_rate_init': [.001, .01, .1]}
-        self.clf = GridSearchCV(self.clf, params, cv=cv, n_jobs=n_jobs)
+        from .mlp_train import DeviceGridSearchCV, DeviceMLPClassifier
+        # a device estimator's fits train together on the GPU (DeviceGridSearchCV ignores n_jobs)
+        search = DeviceGridSearchCV if isinstance(self.clf, DeviceMLPClassifier) else GridSearchCV
+        self.clf = search(self.clf, params, cv=cv, n_jobs=n_jobs)
         self._head = None
 
     def save_model(self, model_file=None):

@@ -279,6 +279,44 @@ int ie_mlp_train_last_epoch_ms(ie_mlp_train* h, float* ms);
 int ie_debug_mlp_train_step(ie_mlp_train* h, int32_t mode, const int32_t* rows, int32_t b, const double* consts,
                             const float* grads, float* out, int64_t cap, double* loss);
 
+/* Group trainer: n_models fits of one architecture (dims) and one batch size, trained in lockstep -- the fits of a grid
+ * search (code_intelligence_b200/mlp_train.py DeviceGridSearchCV).  X [n, D_in] and Y [n, n_labels] are resident once;
+ * each model trains on rows of them that the caller names (its fold, its early-stopping split) and keeps its own
+ * parameters, Adam moments, snapshot, constants (alpha, beta_1, beta_2, epsilon) and workspace.  Every stage of a step
+ * is one launch for all models whose batch has the same size, so a step costs the launches of one ie_mlp_train step
+ * whatever the group size.  Each model's results are bit-identical to an ie_mlp_train handle given the same rows,
+ * parameters and learning rates: its tiles and reductions run the same instructions over the same partitions.  A model
+ * whose values turn non-finite affects no other.  Host pointers only; every call returns when its work is done. */
+typedef struct ie_mlp_group ie_mlp_group;
+/* Device bytes one model of such a group takes, and the models that fit in `fraction` of the device's free memory
+ * (at most 65535, the largest n_models ie_mlp_group_create accepts). */
+int ie_mlp_group_capacity(int32_t n_layers, const int32_t* dims, int32_t batch_size, int32_t device, double fraction,
+                          int64_t* bytes_per_model, int32_t* max_models);
+int ie_mlp_group_create(int32_t n_layers, const int32_t* dims, int32_t n_models, int32_t batch_size, int32_t device,
+                        ie_mlp_group** out);
+void ie_mlp_group_destroy(ie_mlp_group* h);
+/* Shared data X [n, D_in] f32 and Y [n, n_labels] u8; non-finite X is refused. */
+int ie_mlp_group_set_data(ie_mlp_group* h, const float* X, const uint8_t* Y, int64_t n);
+/* Model `model`'s layer parameters (resets its Adam moments, t = 0) / current (best 0) or snapshot (best 1) parameters. */
+int ie_mlp_group_set_layer(ie_mlp_group* h, int32_t model, int32_t layer, const float* coef, const float* intercept);
+int ie_mlp_group_get_layer(ie_mlp_group* h, int32_t model, int32_t layer, int32_t best, float* coef, float* intercept);
+/* Model `model`'s alpha and Adam constants. */
+int ie_mlp_group_set_hyper(ie_mlp_group* h, int32_t model, double alpha, double beta_1, double beta_2, double epsilon);
+/* Model `model`'s validation rows (indices into X), n_val >= 1. */
+int ie_mlp_group_set_validation(ie_mlp_group* h, int32_t model, const int32_t* rows, int64_t n_val);
+/* One epoch of the models models[0 .. n_active): model i trains on rows[i] (n_rows[i] indices into X, in step order, the
+ * rows of all models concatenated), steps k = 0 .. ceil(n_rows[i] / batch_size) - 1 with learning rates lr (each model's
+ * steps concatenated) and batch losses out in losses (same layout).  No host synchronisation between steps. */
+int ie_mlp_group_epoch(ie_mlp_group* h, int32_t n_active, const int32_t* models, const int64_t* n_rows,
+                       const int32_t* rows, const double* lr, double* losses);
+/* Probabilities [n_val, n_labels] f32 of model `model`'s validation rows. */
+int ie_mlp_group_validation_proba(ie_mlp_group* h, int32_t model, float* probs);
+/* restore 0: snapshot model `model`'s parameters as its best; 1: make its snapshot current again. */
+int ie_mlp_group_snapshot(ie_mlp_group* h, int32_t model, int32_t restore);
+/* Kernels launched by this handle so far / device time (CUDA events) of the last ie_mlp_group_epoch. */
+int64_t ie_mlp_group_launch_count(const ie_mlp_group* h);
+int ie_mlp_group_last_epoch_ms(ie_mlp_group* h, float* ms);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,5 +1,6 @@
 """Development aid: a tiny run of every kernel (persistent recurrent kernel, per-timestep fallback, both GEMMs, gather /
-table / finalize, MLP head) for compute-sanitizer (memcheck / racecheck / synccheck), checked against the oracle.
+table / finalize, MLP head, the label-MLP trainer and its group form) for compute-sanitizer (memcheck / racecheck /
+synccheck), checked against the oracle or, for the group trainer, against the single-model fits.
 
     IE_SPIN_LIMIT_MS=600000 compute-sanitizer --tool memcheck python tools/sanitize_tiny.py
 """
@@ -41,4 +42,23 @@ X = rng.standard_normal((300, 24)).astype(np.float32)
 head = MLPHead(coefs, ints)
 assert np.abs(head.predict_proba(X) - N.mlp_forward(X, coefs, ints)).max() < 5e-3
 head.close()
+import warnings
+
+from code_intelligence_b200 import mlp_train as MT
+# group trainer: 2 shapes x 3 models over stacked slots, short last batches of two sizes, early stopping, each fit
+# equal to its own single-handle fit
+Xg = rng.standard_normal((150, 40)).astype(np.float32)
+Yg = (Xg[:, :3] > 0).astype(int)
+folds = [np.arange(0, 100), np.arange(50, 150), np.arange(0, 101)]
+jobs = [(MT.DeviceMLPClassifier(hidden_layer_sizes=h, max_iter=3, random_state=s, batch_size=32,
+                                early_stopping=s == 1), f) for h in ((24,), (20, 12)) for s, f in enumerate(folds)]
+with warnings.catch_warnings():
+    warnings.simplefilter("ignore")
+    trained = MT._train_groups(jobs, Xg, Yg)
+    for (est, rows), rec in zip(jobs, trained):
+        want = MT.DeviceMLPClassifier(**est.get_params()).fit(Xg[rows], Yg[rows])
+        assert rec.error is None and rec.est.loss_curve_ == want.loss_curve_
+        assert all(np.array_equal(a, b) for a, b in zip(rec.est.coefs_ + rec.est.intercepts_,
+                                                          want.coefs_ + want.intercepts_))
+print("group trainer: 6 fits equal to their single fits", flush=True)
 print("sanitize_tiny ok")

@@ -96,6 +96,17 @@ PROTOTYPES = {
     "ie_mlp_group_snapshot": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "ie_mlp_group_launch_count": (C.c_int64, [C.c_void_p]),
     "ie_mlp_group_last_epoch_ms": (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
+    "ie_clas_window": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
+    "ie_clas_create": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_void_p)]),
+    "ie_clas_destroy": (None, [C.c_void_p]),
+    "ie_clas_load_stage": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
+                                     C.c_void_p, C.c_void_p]),
+    "ie_clas_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                  C.c_void_p, C.c_int32, C.c_void_p]),
+    "ie_clas_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                               C.c_int32, C.c_void_p]),
+    "ie_clas_check_errors": (C.c_int, [C.c_void_p]),
+    "ie_clas_launch_count": (C.c_int64, [C.c_void_p]),
 }
 
 _lib = None

@@ -285,4 +285,17 @@ struct GroupGemmArgs {
 };
 cudaError_t launch_group_gemm(const GroupGemmArgs& g, cudaStream_t stream);
 
+// ---- text classifier (clas.cu) ---------------------------------------------------------------------------------------
+// raw [B, T, ld] f32 states, ids [B, T] int64, window [starts[b], ends[b]) -> out [B, 3*e_sz] = [last | max | avg] with
+// fastai's pad mask (ids == pad_idx).  A window outside [0, T], empty or all pad raises err[2] and gives a NaN row.
+// enc_err (optional): the encoder's error words, OR-ed into err[0] (token id) and err[1] (wait timeout).
+cudaError_t launch_clas_pool(const float* raw, long long ld, int B, int T, const int64_t* ids, const int* starts,
+                             const int* ends, int e_sz, int pad_idx, float* out, const int* enc_err, int* err,
+                             cudaStream_t stream);
+// y [rows, N] = act(fma(x, alpha, beta) . W^T + bias), x [rows, K], W [N, K] (torch Linear layout), relu 0/1
+cudaError_t launch_clas_linear(const float* x, int rows, int K, const float* alpha, const float* beta, const float* W,
+                               const float* bias, int N, int relu, float* y, cudaStream_t stream);
+// p [rows, N] = sigmoid(z) (softmax 0) or the max-subtracted softmax of each row (softmax 1)
+cudaError_t launch_clas_activate(const float* z, int rows, int N, int softmax, float* p, cudaStream_t stream);
+
 }  // namespace ie

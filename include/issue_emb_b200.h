@@ -317,6 +317,45 @@ int ie_mlp_group_snapshot(ie_mlp_group* h, int32_t model, int32_t restore);
 int64_t ie_mlp_group_launch_count(const ie_mlp_group* h);
 int ie_mlp_group_last_epoch_ms(ie_mlp_group* h, float* ms);
 
+/* Text classifier.  Replaces the model fastai's text_classifier_learner builds on the AWD-LSTM encoder
+ * (Issue_Embeddings/notebooks/06_FineTune.ipynb: get_text_classifier = SequentialRNN(MultiBatchEncoder,
+ * PoolingLinearClassifier), fastai 1.0.53) in eval mode, as learn.predict / learn.model(x) run it:
+ *   encoder  the borrowed ie_encoder's states o [B, T, emb_sz] of ids [B, T] (zero initial state, every step run,
+ *            pads included -- fastai's batched forward over pad_collate(pad_first=True) batches)
+ *   pool     per row b over the window [starts[b], ends[b]) of W steps, mask = (ids == pad_idx):
+ *            [last | max | avg] = o[b, ends[b]-1], max of the unmasked steps, (sum of the unmasked steps / W) *
+ *            f32(W / (W - n_masked)) -- fastai's masked_concat_pool on the window of kept bptt chunks (ie_clas_window)
+ *   head     per stage k: BatchNorm1d(dims[k]) with the running statistics, Linear(dims[k], dims[k+1]), ReLU except on
+ *            the last stage; then sigmoid (IE_CLAS_SIGMOID, multi-label) or softmax (IE_CLAS_SOFTMAX) of the logits.
+ * dims [n_stages + 1] = {3*emb_sz, hidden..., n_class}.  The handle borrows the encoder (weights, workspace, stream,
+ * serialisation): destroy it before the encoder.  Windows are validated on the host before any launch with host
+ * pointers (IE_ERR_INVALID for one outside [0, T], empty, or entirely pad); with IE_FLAG_DEVICE_PTRS such a row is NaN and
+ * ie_clas_check_errors() reports it, with the encoder's own token-id and wait errors.  B <= ie_encoder_max_batch(enc);
+ * rows are encoded in groups whose f32 states fit 4 GB (one row at a time beyond). */
+#define IE_CLAS_SIGMOID 0
+#define IE_CLAS_SOFTMAX 1
+typedef struct ie_clas ie_clas;
+/* First kept step of a sequence of sl steps: MultiBatchEncoder(bptt, max_len) keeps chunk i (i = 0, bptt, ...) when
+ * i > sl - max_len.  IE_ERR_INVALID when no chunk is kept (only possible with max_len <= bptt).  Host only. */
+int ie_clas_window(int32_t sl, int32_t bptt, int32_t max_len, int32_t* start);
+int ie_clas_create(ie_encoder* enc, int32_t n_stages, const int32_t* dims, int32_t activation, ie_clas** out);
+void ie_clas_destroy(ie_clas* c);
+/* Stage `stage`: BatchNorm1d weight, bias (each may be NULL: 1 / 0), running_mean, running_var [dims[stage]], eps;
+ * Linear weight [dims[stage+1], dims[stage]] (torch layout) and bias [dims[stage+1]].  Host f32; non-finite refused. */
+int ie_clas_load_stage(ie_clas* c, int32_t stage, const float* bn_weight, const float* bn_bias, const float* bn_mean,
+                       const float* bn_var, double eps, const float* lin_weight, const float* lin_bias);
+/* ids [B, T] int64, starts / ends [B] int32 -> out [B, n_class] f32 (activated); logits [B, n_class] (optional, NULL). */
+int ie_clas_forward(ie_clas* c, const int64_t* ids, const int32_t* starts, const int32_t* ends, int32_t B, int32_t T,
+                    float* out, float* logits, int32_t flags, void* stream);
+/* The pool alone: pooled [B, 3*emb_sz] f32 = [last | max | avg], the head's input. */
+int ie_clas_pool(ie_clas* c, const int64_t* ids, const int32_t* starts, const int32_t* ends, int32_t B, int32_t T,
+                 float* pooled, int32_t flags, void* stream);
+/* Device-side errors of the last call on this handle (waits for it; clears them): IE_ERR_CUDA, IE_ERR_TOKEN or
+ * IE_ERR_INVALID (a bad or all-pad window in device-pointer mode). */
+int ie_clas_check_errors(ie_clas* c);
+/* Kernels this handle has launched (pool, head stages, activation); the encoder's count its own. */
+int64_t ie_clas_launch_count(const ie_clas* c);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,6 +1,7 @@
 """ORACLE (test infrastructure, NOT product code) for the text classifier: fastai 1.0.53's text_classifier_learner on
 the AWD-LSTM encoder (Issue_Embeddings/notebooks/06_FineTune.ipynb) in eval mode, restated on torch modules, plus the
-float64 restatement of the device's pool and head with their per-element bounds.
+float64 restatement of the device's pool and head with their per-element bounds, and the exact float32 restatement of
+the same kernels (their bits) with relative bounds for the activations.
 
 fastai is not installed; the semantics below are restated from fastai 1.0.53's published source (text/learner.py,
 text/models/awd_lstm.py, layers.py), nothing is copied:
@@ -239,3 +240,151 @@ def head_f64(x: np.ndarray, stages: Sequence[dict], activation: str = "sigmoid",
         ep = p * (2 * ez.max(1, keepdims=True) + U * np.abs(d) + U * np.abs(d).max(1, keepdims=True)
                   + (N + 8) * U) * 1.01 + 2.0 ** -126
     return z, ez, p, ep
+
+
+# ---------------------------------------------------------------------------------------------------
+# exact float32 restatement of csrc/clas.cu: the device's pool and logits bit for bit
+# ---------------------------------------------------------------------------------------------------
+# Every function below takes and returns torch tensors and runs on the CPU or the GPU alike.  Values are held in float64
+# and rounded to float32 after each operation, one eager op per step, so nothing contracts into an fma.  For +, -, *, /
+# and sqrt that double rounding is innocuous: 53 >= 2 * 24 + 2 bits, so f32(f64(a op b)) is the correctly rounded f32
+# result (Figueroa, "When is double rounding innocuous?", 1995).  An fma has no such guarantee and goes through fma_f32.
+
+def _f32(t: torch.Tensor) -> torch.Tensor:
+    """Round to the nearest f32 (ties to even), kept in float64."""
+    return t.to(torch.float32).to(torch.float64)
+
+
+def _t64(a, device=None) -> torch.Tensor:
+    t = torch.as_tensor(a, device=device)
+    if t.dtype != torch.float32 and t.dtype != torch.float64:
+        raise TypeError(f"expected float32 values, got {t.dtype}")
+    return t.to(torch.float64)
+
+
+def fma_f32(a, b, c) -> torch.Tensor:
+    """The correctly rounded f32 fma(a, b, c) of f32 values (held in float64), elementwise with broadcasting.
+
+    The product of two f32 values is exact in float64; s = p + c is rounded once and TwoSum gives its exact error.  When
+    that error is non-zero and s has an even last bit, s steps one float64 ulp toward the error: s is then p + c rounded
+    to odd at 53 bits, and rounding a round-to-odd value of 53 >= 24 + 2 bits to f32 is the correctly rounded result
+    (Boldo & Melquiond, 2008).  The plain f32(f64(a * b) + c) rounds twice and can land on the wrong side of an f32
+    midpoint: a = b = 1 + 2^-12, c = 2^-80 gives the midpoint 1 + 2^-11 + 2^-24 after the first rounding, which then goes
+    down to even while the exact sum lies above it."""
+    a, b, c = torch.broadcast_tensors(_t64(a), _t64(b), _t64(c))
+    p = a * b
+    s = p + c
+    bv = s - p
+    err = (p - (s - bv)) + (c - bv)
+    even = (s.view(torch.int64) & 1) == 0
+    toward = torch.where(err > 0, torch.full_like(s, float("inf")), torch.full_like(s, -float("inf")))
+    s = torch.where((err != 0) & even & torch.isfinite(s), torch.nextafter(s, toward), s)
+    return _f32(s)
+
+
+def bn_fold_f32(stage: dict, eps: float = 1e-5, device=None):
+    """(alpha, beta) float64 tensors holding what ie_clas_load_stage computes on the host in f32:
+    alpha = f32(f32(1 / f32(sqrt(f32(var + f32(eps))))) * w), beta = fma(-mean, alpha, b)."""
+    w, b, m, v = (_t64(np.asarray(stage[n], np.float32), device) for n in ("bn_weight", "bn_bias", "bn_mean", "bn_var"))
+    invstd = _f32(1.0 / _f32(torch.sqrt(_f32(v + float(np.float32(eps))))))
+    alpha = _f32(invstd * w)
+    return alpha, fma_f32(-m, alpha, b)
+
+
+def pool_f32(raw, ids, starts, ends, pad_idx: int, pairwise: bool = False) -> torch.Tensor:
+    """clas_pool_kernel bit for bit: raw [B, T, E] f32 states, ids [B, T], window [starts[b], ends[b]) -> [B, 3E]
+    float64 holding f32 values [last | max | avg].  last = raw[e - 1] (masked or not); max over the unmasked steps; the
+    unmasked steps summed in step order from +0, mean = f32(sum / f32(W)), factor = f32(f32(W) / f32(W - n_masked)),
+    avg = f32(mean * factor).  ``pairwise=True`` is a negative control: the same sum over two accumulators (even and odd
+    steps of the window) added at the end, an order the kernel must not have."""
+    raw = _t64(raw)
+    dev = raw.device
+    B, T, E = raw.shape
+    ids = torch.as_tensor(ids, device=dev)
+    st = torch.as_tensor(starts, device=dev).long()
+    en = torch.as_tensor(ends, device=dev).long()
+    if bool(((st < 0) | (en > T) | (st >= en)).any()):
+        raise ValueError("a window is empty or outside [0, T]")
+    t = torch.arange(T, device=dev)
+    inside = (t[None, :] >= st[:, None]) & (t[None, :] < en[:, None])
+    keep = inside & (ids != pad_idx)
+    n = keep.sum(1)
+    if bool((n == 0).any()):
+        raise ValueError("a window is entirely pad")
+    rows = torch.arange(B, device=dev)
+    last = raw[rows, en - 1]
+    mx = torch.where(keep[:, :, None], raw, torch.full_like(raw, -float("inf"))).amax(1)
+    acc = [torch.zeros(B, E, dtype=torch.float64, device=dev) for _ in range(2)]
+    odd = (t[None, :] - st[:, None]) % 2 == 1
+    for i in range(int(st.min()), int(en.max())):
+        sels = (keep[:, i] & ~odd[:, i], keep[:, i] & odd[:, i]) if pairwise else (keep[:, i],)
+        for j, sel in enumerate(sels):
+            acc[j] = torch.where(sel[:, None], _f32(acc[j] + raw[:, i]), acc[j])
+    total = _f32(acc[0] + acc[1]) if pairwise else acc[0]
+    w = _f32((en - st).to(torch.float64))[:, None]
+    mean = _f32(total / w)
+    factor = _f32(w / _f32(n.to(torch.float64))[:, None])
+    return torch.cat([last, mx, _f32(mean * factor)], 1)
+
+
+def linear_f32(x, alpha, beta, W, bias, relu: bool, reverse: bool = False) -> torch.Tensor:
+    """clas_linear_kernel bit for bit: x [B, K] f32 -> [B, N] float64 holding f32 values.  xn = fma(x, alpha, beta);
+    acc = +0, then acc = fma(xn[k], W[j, k], acc) for k = 0 .. K - 1; v = f32(acc + bias[j]); ReLU as the kernel writes
+    it (v < 0 -> +0, so NaN and -0 pass through).  ``reverse=True`` is a negative control: the chain from k = K - 1 down."""
+    x = _t64(x)
+    dev = x.device
+    alpha, beta, bias = (_t64(a, dev) for a in (alpha, beta, bias))
+    W = _t64(W, dev)
+    xn = fma_f32(x, alpha[None, :], beta[None, :])
+    K = xn.shape[1]
+    acc = torch.zeros(x.shape[0], W.shape[0], dtype=torch.float64, device=dev)
+    Wt = W.t().contiguous()
+    for k in (range(K - 1, -1, -1) if reverse else range(K)):
+        acc = fma_f32(xn[:, k, None], Wt[k][None, :], acc)
+    v = _f32(acc + bias[None, :])
+    if relu:
+        v = torch.where(v < 0, torch.zeros_like(v), v)
+    return v
+
+
+def head_f32(pooled, stages: Sequence[dict], eps: float = 1e-5, reverse: bool = False) -> torch.Tensor:
+    """The exact logits [B, n_class] (float64 holding f32 values) of the head on the pooled input: per stage the
+    BatchNorm fold of ``bn_fold_f32`` and ``linear_f32``, ReLU on every stage but the last."""
+    x = _t64(pooled)
+    for k, st in enumerate(stages):
+        alpha, beta = bn_fold_f32(st, eps, x.device)
+        W = torch.as_tensor(np.asarray(st["weight"], np.float32), device=x.device)
+        b = torch.as_tensor(np.asarray(st["bias"], np.float32), device=x.device)
+        x = linear_f32(x, alpha, beta, W, b, relu=k < len(stages) - 1, reverse=reverse)
+    return x
+
+
+def sigmoid_bound(z):
+    """(p64, bound) for clas_activate_kernel's sigmoid on exact logits z (f32 values): |p_device - p64| <= bound.
+
+    The device computes e = expf(-z), q = f32(1 + e), p = f32(1 / q).  expf is within 2 ulp (CUDA C++ Programming Guide,
+    single-precision mathematical functions), at most 4u |e| for a normal e; p = 1 / (1 + e) has dp / p = -(e / (1 + e))
+    de / e, so that is at most 4u relative in p.  The add and the division add u each: 6u p to first order, times 1.01
+    for the second-order terms.  Where -z > 88.72 expf overflows to inf and the device gives 0 for a p below 3e-39, and a
+    subnormal e or p is off by at most a subnormal ulp: the absolute term 2^-126 covers both."""
+    z = _t64(z)
+    p = 1.0 / (1.0 + torch.exp(-z))
+    return p, 1.01 * 6 * U * p + 2.0 ** -126
+
+
+def softmax_bound(z):
+    """(p64, bound) for clas_activate_kernel's softmax on exact logits z [B, N] (f32 values), row by row.
+
+    Device: m = max z (exact); d_j = f32(z_j - m), off by at most u |d_j|, which moves expf's result by a relative
+    u |d_j| (first order); e_j = expf(d_j) adds 4u (2 ulp); each lane sums its L = ceil(N / 32) terms from +0 (L - 1
+    roundings: the first add is exact), the xor butterfly adds five more, all of positive terms: the sum S is within
+    (L + 4) u + 4u + u max|d| relative.  p_j = f32(e_j / S) adds u to e_j's own 4u + u |d_j|.  So p_j is within
+    p_j ((L + 13) u + u |d_j| + u max|d|) to first order (times 1.01), plus 2^-126 absolute for terms expf flushes to a
+    subnormal or zero once d < -87.3."""
+    z = _t64(z)
+    d = z - z.max(1, keepdim=True).values
+    e = torch.exp(d)
+    p = e / e.sum(1, keepdim=True)
+    L = -(-z.shape[1] // 32)
+    ad = d.abs()
+    return p, 1.01 * p * ((L + 13) * U + U * ad + U * ad.max(1, keepdim=True).values) + 2.0 ** -126

@@ -1,9 +1,11 @@
 """CPU tests of the text classifier's host side: fastai's window rule (oracle and ie_clas_window), the oracle against a
 literal MultiBatchEncoder run, the head-layout inference of a fastai state dict, the refusals, the plain-C declarations
-and the ptxas figures of csrc/clas.cu."""
+and the ptxas figures of csrc/clas.cu; the exact f32 restatement of the pool and head (its fma against exact rationals,
+its agreement with the float64 restatement's bounds, and the negative controls the GPU checks rely on)."""
 import os
 import re
 import subprocess
+from fractions import Fraction
 
 import numpy as np
 import pytest
@@ -119,9 +121,9 @@ def test_head_layout_refusals():
 
 def test_bn_fold_restates_torch_eval_batchnorm():
     """The device folds eval BatchNorm1d as torch's CPU kernel does: alpha = (1 / sqrt(var + eps)) * w,
-    beta = fma(-mean, alpha, b), y = fma(x, alpha, beta).  Checked on this torch: where the fma forms are evaluated
-    exactly (float64 then one rounding), at least 99.9 % of the elements match torch's bits and the rest differ by one
-    ulp (torch's CPU kernel may be vectorised differently on other instruction sets)."""
+    beta = fma(-mean, alpha, b), y = fma(x, alpha, beta) -- oracle.text_clas_ref.bn_fold_f32 and fma_f32.  Checked on
+    this torch: at least 99.9 % of the elements match torch's bits and the rest differ by one ulp (torch's CPU kernel
+    may be vectorised differently on other instruction sets)."""
     torch.manual_seed(0)
     n = 2048
     bn = torch.nn.BatchNorm1d(n).eval()
@@ -132,12 +134,204 @@ def test_bn_fold_restates_torch_eval_batchnorm():
         bn.running_var.copy_(torch.rand(n) * 5 + 1e-3)
     x = torch.randn(32, n) * 4
     y = bn(x).detach().numpy()
-    w, b, m, v = (t.detach().numpy() for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
-    alpha = (np.float32(1) / np.sqrt(v + np.float32(1e-5))) * w
-    beta = (b.astype(np.float64) - m.astype(np.float64) * alpha).astype(np.float32)
-    got = (x.numpy().astype(np.float64) * alpha + beta).astype(np.float32)
+    stage = dict(bn_weight=bn.weight.detach().numpy(), bn_bias=bn.bias.detach().numpy(),
+                 bn_mean=bn.running_mean.numpy(), bn_var=bn.running_var.numpy())
+    alpha, beta = TR.bn_fold_f32(stage, bn.eps)
+    got = TR.fma_f32(x, alpha[None, :], beta[None, :]).numpy().astype(np.float32)
     assert (got == y).mean() >= 0.999
     assert np.abs(got.view(np.int32) - y.view(np.int32)).max() <= 1
+    # the fold's own rounding points: alpha is the f32 product of the f32 reciprocal square root and w
+    v32 = stage["bn_var"] + np.float32(bn.eps)
+    np.testing.assert_array_equal(alpha.numpy().astype(np.float32),
+                                  (np.float32(1) / np.sqrt(v32)).astype(np.float32) * stage["bn_weight"])
+
+
+# ------------------------------------------------------------------------- exact f32 restatement (oracle/text_clas_ref)
+def _round_f32(x: Fraction) -> float:
+    """A non-zero rational rounded to the nearest f32, ties to even (overflow to inf), as a float."""
+    sgn = -1 if x < 0 else 1
+    x = abs(x)
+    e = x.numerator.bit_length() - x.denominator.bit_length()
+    if x < Fraction(2) ** e:
+        e -= 1                                              # now 2^e <= x < 2^(e + 1)
+    q = Fraction(2) ** (max(e, -126) - 23)                  # the f32 spacing there (subnormal below 2^-126)
+    v = round(x / q) * q                                    # Fraction rounds half to even
+    if v >= Fraction(2) ** 128:
+        return sgn * float("inf")
+    return sgn * float(v)
+
+
+def _fma_exact(a: np.float32, b: np.float32, c: np.float32) -> np.float32:
+    """fma(a, b, c) from exact rationals: one rounding of a b + c; an exact zero is -0 only when a b and c are both
+    -0 (IEEE 754 round to nearest)."""
+    s = Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c))
+    if s != 0:
+        return np.float32(_round_f32(s))
+    prod_neg = np.signbit(a) != np.signbit(b)
+    both_neg_zero = a * b == 0 and prod_neg and c == 0 and np.signbit(c)
+    return np.float32(-0.0 if both_neg_zero else 0.0)
+
+
+def _bits(x) -> np.ndarray:
+    return np.asarray(x, np.float32).view(np.uint32)
+
+
+def _check_fma(a, b, c):
+    a, b, c = (np.asarray(t, np.float32) for t in (a, b, c))
+    got = TR.fma_f32(torch.as_tensor(a), torch.as_tensor(b), torch.as_tensor(c)).numpy().astype(np.float32)
+    want = np.array([_fma_exact(*t) for t in zip(a, b, c)], np.float32)
+    bad = np.flatnonzero(_bits(got) != _bits(want))
+    assert bad.size == 0, [(a[i], b[i], c[i], got[i], want[i]) for i in bad[:5]]
+
+
+def _f32_values(rng, n, lo, hi):
+    """Random f32 values of random sign with exponents uniform in [lo, hi]."""
+    m = rng.uniform(1, 2, n)
+    return (rng.choice([-1.0, 1.0], n) * m * 2.0 ** rng.integers(lo, hi + 1, n)).astype(np.float32)
+
+
+def test_fma_f32_is_correctly_rounded_on_random_triples():
+    rng = np.random.default_rng(0)
+    n = 6000
+    a, b = _f32_values(rng, n, -20, 20), _f32_values(rng, n, -20, 20)
+    c = _f32_values(rng, n, -45, 45)
+    _check_fma(a, b, c)
+    # near-cancellation: c within a few ulp of -a b, so the result is the product's low bits
+    p = (a.astype(np.float64) * b).astype(np.float32)
+    near = np.nextafter(-p, rng.choice([-np.inf, np.inf], n).astype(np.float32)).astype(np.float32)
+    _check_fma(a, b, near)
+    _check_fma(a, b, -p)
+
+
+def test_fma_f32_at_an_f32_midpoint_where_plain_double_rounding_fails():
+    """a = b = 1 + 2^-12: a b = 1 + 2^-11 + 2^-24 is the midpoint of two f32 values.  With c = +2^-80 the exact sum lies
+    above it and the fma rounds up; f32(f64(a b) + c) loses c in the first rounding and then rounds the tie down to
+    even.  With c = -2^-80 both round down."""
+    a = np.float32(1 + 2.0 ** -12)
+    for sgn in (1, -1):
+        c = np.float32(sgn * 2.0 ** -80)
+        want = _fma_exact(a, a, c)
+        got = TR.fma_f32(torch.tensor([a]), torch.tensor([a]), torch.tensor([c])).numpy().astype(np.float32)[0]
+        assert _bits(got) == _bits(want)
+        plain = np.float32(np.float64(a) * np.float64(a) + np.float64(c))
+        assert (plain == want) == (sgn < 0), (sgn, plain, want)
+    assert _fma_exact(a, a, np.float32(2.0 ** -80)) == np.float32(1 + 2.0 ** -11 + 2.0 ** -23)
+
+
+def test_fma_f32_signed_zeros_subnormals_and_exponent_gaps():
+    z, one = np.float32(0.0), np.float32(1.0)
+    a, b, c = [], [], []
+
+    def add(x, y, w):
+        a.append(x), b.append(y), c.append(w)
+
+    for x, y, w in [(one, one, -one), (-one, one, one), (z, one, -z), (-z, one, -z), (z, -one, -z), (-z, -one, -z),
+                    (z, one, z), (np.float32(3), np.float32(5), np.float32(-15)), (np.float32(1.5), np.float32(-2),
+                                                                                      np.float32(3))]:
+        add(x, y, w)                                        # exact cancellation: +0, or -0 only from -0 + -0
+    rng = np.random.default_rng(1)
+    sub = np.float32(2.0 ** -149)
+    for _ in range(800):
+        x, y = _f32_values(rng, 2, -75, -60)                # product 2^-150 .. 2^-120: subnormal or just normal
+        add(x, y, np.float32(rng.integers(-2 ** 20, 2 ** 20)) * sub)
+        x, y = _f32_values(rng, 2, -10, 10)                 # a tiny or huge c against a moderate product
+        add(x, y, _f32_values(rng, 1, -140, -100)[0])
+        add(x, y, _f32_values(rng, 1, 60, 100)[0])
+        x, y = _f32_values(rng, 2, 55, 63)                  # product near the f32 overflow threshold
+        add(x, y, _f32_values(rng, 1, 100, 127)[0])
+    _check_fma(a, b, c)
+    zeros = TR.fma_f32(torch.tensor([1.0, -0.0]), torch.tensor([-1.0, 1.0]), torch.tensor([1.0, -0.0]))
+    assert list(np.signbit(zeros.numpy())) == [False, True]
+
+
+def _stages(rng, dims, x):
+    """Random head stages with BatchNorm statistics calibrated on x (float64 forward between stages)."""
+    stages = []
+    a = x.astype(np.float64)
+    for k, (K, N) in enumerate(zip(dims[:-1], dims[1:])):
+        st = dict(bn_weight=(1 + 0.2 * rng.standard_normal(K)).astype(np.float32),
+                  bn_bias=(0.1 * rng.standard_normal(K)).astype(np.float32),
+                  bn_mean=a.mean(0).astype(np.float32), bn_var=(a.var(0) + 1e-4).astype(np.float32),
+                  weight=(rng.standard_normal((N, K)) / np.sqrt(K)).astype(np.float32),
+                  bias=(0.1 * rng.standard_normal(N)).astype(np.float32))
+        stages.append(st)
+        xn = (a - st["bn_mean"]) / np.sqrt(st["bn_var"].astype(np.float64) + 1e-5) * st["bn_weight"] + st["bn_bias"]
+        a = xn @ st["weight"].T.astype(np.float64) + st["bias"]
+        if k < len(dims) - 2:
+            a = np.maximum(a, 0)
+    return stages
+
+
+def _pool_inputs(rng, B, T, E, pad=1):
+    raw = np.tanh(rng.standard_normal((B, T, E)) * 1.5).astype(np.float32)
+    ids = rng.integers(2, 100, size=(B, T))
+    starts = np.array([TR.window_start(T)] * B, np.int32)
+    ends = np.full(B, T, np.int32)
+    ids[0, :7] = pad                                        # pads in front of the window's first kept step
+    ids[1, T // 2] = pad                                    # inside
+    ids[2, -1] = pad                                        # on the last step
+    ends[3] = T - 5                                         # a shorter window, right padding after it
+    ids[3, T - 5:] = pad
+    starts[3] = TR.window_start(T - 5)
+    return raw, ids, starts, ends
+
+
+@pytest.mark.parametrize("T,E", [(150, 96), (600, 800)])
+def test_exact_pool_lies_within_the_float64_bound(T, E):
+    rng = np.random.default_rng(T)
+    raw, ids, starts, ends = _pool_inputs(rng, 4, T, E)
+    got = TR.pool_f32(raw, ids, starts, ends, 1).numpy()
+    assert np.array_equal(got, got.astype(np.float32))     # f32 values
+    last, mx, avg, bound = TR.pool_f64(raw, ids, starts, ends, 1)
+    np.testing.assert_array_equal(got[:, :E], last)
+    np.testing.assert_array_equal(got[:, E:2 * E], mx)
+    err = np.abs(got[:, 2 * E:] - avg)
+    assert (err <= bound).all(), (err / bound).max()
+    assert (err > 0).mean() > 0.3                           # the f32 sum does round
+
+
+@pytest.mark.parametrize("dims", [[288, 50, 3], [2400, 50, 28], [2400, 129, 33, 5]])
+def test_exact_head_lies_within_the_float64_bound(dims):
+    rng = np.random.default_rng(len(dims) + dims[0])
+    x = np.tanh(rng.standard_normal((24, dims[0]))).astype(np.float32)
+    stages = _stages(rng, dims, x)
+    z = TR.head_f32(x, stages).numpy()
+    assert np.array_equal(z, z.astype(np.float32))
+    z64, ez, _, _ = TR.head_f64(x, stages)
+    assert (np.abs(z - z64) <= ez).all(), (np.abs(z - z64) / ez).max()
+    assert np.std(z64) > 0.05
+
+
+def test_reordered_sums_differ_from_the_exact_restatement():
+    """The negative controls the GPU checks rest on: at the 06 shape a reversed k chain (K = 2400) and a two-accumulator
+    pool sum give other bits in a non-trivial fraction of the elements, so equality with the forward restatement pins
+    the order."""
+    rng = np.random.default_rng(7)
+    x = np.tanh(rng.standard_normal((32, 2400))).astype(np.float32)
+    stages = _stages(rng, [2400, 50], x)
+    fwd = TR.head_f32(x, stages).numpy()
+    rev = TR.head_f32(x, stages, reverse=True).numpy()
+    assert (fwd != rev).mean() > 0.2, (fwd != rev).mean()
+    raw, ids, starts, ends = _pool_inputs(rng, 4, 512, 800)
+    fwd = TR.pool_f32(raw, ids, starts, ends, 1).numpy()
+    pw = TR.pool_f32(raw, ids, starts, ends, 1, pairwise=True).numpy()
+    np.testing.assert_array_equal(fwd[:, :1600], pw[:, :1600])     # last and max do not depend on the order
+    assert (fwd[:, 1600:] != pw[:, 1600:]).mean() > 0.2, (fwd[:, 1600:] != pw[:, 1600:]).mean()
+
+
+def test_activation_bounds_on_exact_logits():
+    """The relative bounds hold for the float32 torch forms on the same logits (a stand-in for the device: a correctly
+    rounded exp is within them) and are tight enough to see a 1e-6 probability off by 1 %."""
+    z = torch.linspace(-110, 110, 4001, dtype=torch.float32)
+    p64, bound = TR.sigmoid_bound(z)
+    p32 = (1 / (1 + torch.exp(-z))).double()
+    assert ((p32 - p64).abs() <= bound).all()
+    i = int(torch.argmin((p64 - 1e-6).abs()))
+    assert bound[i] < 0.01 * p64[i]
+    zs = torch.tensor([[0.0, -5.0, -100.0, 3.5, -120.0] * 7], dtype=torch.float32)
+    p64, bound = TR.softmax_bound(zs)
+    assert ((torch.softmax(zs, 1).double() - p64).abs() <= bound).all()
+    assert (bound <= p64 * 1e-4 + 2.0 ** -126).all()
 
 
 def test_clas_abi_from_plain_c(tmp_path):

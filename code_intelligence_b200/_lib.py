@@ -172,17 +172,20 @@ def _debug_gemm(a, b, bias=None, act: int = 0, out_type: int = 0, segs: int = 1,
 
 GATE_FNS = ("sigmoid_fast", "tanh_fast", "sigmoid_acc", "tanh_acc", "sigmoid_ieee", "tanh_ieee")
 CELL_FNS = {"fast": 6, "exp": 7, "ieee": 8}
+LM_MATH_FNS = {"lm_ex2": 9, "lm_log": 10}   # the language-model decoder's ex2.approx.ftz and logf (csrc/lm.cu)
 
 
 def _debug_gates(fn, x):
-    """Test hook ``ie_debug_gates`` on CUDA float32 tensors.  fn a name of GATE_FNS: f(x) elementwise, same shape.
-    fn 'cell_fast' | 'cell_exp' | 'cell_ieee': x [5, n] planes (zi, zf, zg, zo, c_prev) -> [2, n] (c_new, h)."""
+    """Test hook ``ie_debug_gates`` on CUDA float32 tensors.  fn a name of GATE_FNS or LM_MATH_FNS: f(x) elementwise,
+    same shape.  fn 'cell_fast' | 'cell_exp' | 'cell_ieee': x [5, n] planes (zi, zf, zg, zo, c_prev) -> [2, n]
+    (c_new, h)."""
     import torch
     x = x.contiguous()
     if x.dtype != torch.float32 or not x.is_cuda:
         raise ValueError("ie_debug_gates takes a CUDA float32 tensor")
-    if fn in GATE_FNS:
-        code, n, out = GATE_FNS.index(fn), x.numel(), torch.empty_like(x)
+    if fn in GATE_FNS or fn in LM_MATH_FNS:
+        code = GATE_FNS.index(fn) if fn in GATE_FNS else LM_MATH_FNS[fn]
+        n, out = x.numel(), torch.empty_like(x)
     else:
         code = CELL_FNS[fn.removeprefix("cell_")]
         if x.dim() != 2 or x.shape[0] != 5:

@@ -19,14 +19,7 @@ namespace {
 
 constexpr float kLog2e = 1.4426950408889634f;
 
-// 2^x, ex2.approx.ftz.f32 (relative error below 2^-22 outside the flushed range)
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// exp(x - m) for x <= m (0 for x = -inf); m must be finite
+// exp(x - m) through ex2_approx (ptx.cuh) for x <= m (0 for x = -inf); m must be finite
 __device__ __forceinline__ float exp_sub(float x, float m) { return ex2_approx((x - m) * kLog2e); }
 
 // (m, s, arg) <- (m, s, arg) merged with (m2, s2, arg2): max, rescaled sum, argmax with ties to the lower index.

@@ -186,6 +186,17 @@ __global__ void debug_gate_kernel(const float* __restrict__ x, float* __restrict
   }
 }
 
+// the language-model decoder's 2^x (FN 9) and log (FN 10), inlined as lm.cu inlines them: ex2_approx (ptx.cuh) and
+// logf under lm.cu's compiler flags.  One copy of the function per kernel, so that the SASS of FN 10 is logf's alone
+// and can be compared with lm_combine_kernel's.
+template <int FN>
+__global__ void debug_lm_math_kernel(const float* __restrict__ x, float* __restrict__ y, long long n) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+#pragma unroll 1
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
+    y[i] = FN == 9 ? ex2_approx(x[i]) : logf(x[i]);
+}
+
 // in = planes [zi | zf | zg | zo | c_prev] of n values, out = planes [c_new | h]
 template <int GM>
 __global__ void debug_cell_kernel(const float* __restrict__ in, float* __restrict__ out, long long n) {
@@ -269,6 +280,8 @@ cudaError_t launch_debug_gates(int fn, const float* in, float* out, long long n,
     case 6: debug_cell_kernel<kGatesFast><<<g, 256, 0, stream>>>(in, out, n); break;
     case 7: debug_cell_kernel<kGatesExp><<<g, 256, 0, stream>>>(in, out, n); break;
     case 8: debug_cell_kernel<kGatesIeee><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 9: debug_lm_math_kernel<9><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 10: debug_lm_math_kernel<10><<<g, 256, 0, stream>>>(in, out, n); break;
     default: return cudaErrorInvalidValue;
   }
   return cudaGetLastError();

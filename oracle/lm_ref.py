@@ -32,7 +32,7 @@ from . import awd_lstm_ref as R
 from . import device_numerics as DN
 
 U = 2.0 ** -24          # f32 unit roundoff
-EXP_REL = 2.0 ** -21    # ex2.approx.ftz.f32 relative error, stated with a factor 2 of margin (lm.cu ex2_approx)
+EXP_REL = 2.0 ** -21    # ex2.approx.ftz.f32 relative error (lm.cu ex2_approx): twice the 2^-22.7 measured on an H100
 SLICE_TILES = 32        # kernels.h kLmSliceTiles
 
 
@@ -202,6 +202,147 @@ def decoder_f64(h, W, b, targets, segs: int, device=None) -> dict:
     b_nll = torch.where(ign, torch.zeros_like(lse), b_lse + et + U * nll.abs())
     f = lambda x: x.detach().cpu().numpy()
     return dict(lse=f(lse), nll=f(nll), pred=f(pred), margin=f(margin), eps=f(e_row), b_lse=f(b_lse), b_nll=f(b_nll))
+
+
+# ------------------------------------------------------------------------------------------------ the decoder in f32
+# The fused decoder (csrc/lm.cu) bit for bit from the f32 accumulators of h W^T.  Every step is one eager torch op on
+# float32 tensors (IEEE round to nearest, no contraction: torch evaluates each op alone), except the rescale, which the
+# kernel contracts into an fma and which goes through text_clas_ref.fma_f32.  The order below is the one lm.cu's SASS
+# has (tests/test_language_model_reference.py pins it): x - m, then a multiply by log2(e) as f32 (0x3fb8aa3b), then
+# ex2; ts a left-to-right chain of adds; s = fma(s, scale, ts) the only contraction; merge two products and one add.
+LOG2E_F32 = float(np.float32(1.4426950408889634))   # lm.cu kLog2e
+NO_ARG = 0x7fffffff
+EXACT_MUTANTS = ("tiles_desc", "no_fma", "quad_pairs", "slices_desc", "one_lane", "log_f64")
+
+
+def ex2_rn(x: torch.Tensor) -> torch.Tensor:
+    """A correctly rounded stand-in for ex2.approx.ftz.f32: 2^x rounded to f32, results below 2^-126 flushed to 0."""
+    y = torch.exp2(x.double())
+    return torch.where(y < 2.0 ** -126, torch.zeros_like(y), y).float()
+
+
+def logf_rn(x: torch.Tensor) -> torch.Tensor:
+    """A correctly rounded stand-in for logf."""
+    return torch.log(x.double()).float()
+
+
+def _exp_sub(x, m, ex2):
+    """lm.cu exp_sub: ex2(f32(f32(x - m) * log2(e)))."""
+    return ex2((x - m) * torch.tensor(LOG2E_F32, dtype=torch.float32, device=x.device))
+
+
+def _merge(a, b, ex2):
+    """lm.cu merge of partials a = (m, s, arg) and b: max, s = f32(s_a * e_a) + f32(s_b * e_b) (two products, one add),
+    argmax with ties to the lower index; unchanged a where both maxima are -inf."""
+    (m, s, arg), (m2, s2, arg2) = a, b
+    ninf = -math.inf
+    mn = torch.maximum(m, m2)
+    dead = mn == ninf
+    mn0 = torch.where(dead, torch.zeros_like(mn), mn)
+    ea = _exp_sub(torch.where(m == ninf, mn0, m), mn0, ex2)
+    eb = _exp_sub(torch.where(m2 == ninf, mn0, m2), mn0, ex2)
+    pa = torch.where(m == ninf, torch.zeros_like(s), s * ea)
+    pb = torch.where(m2 == ninf, torch.zeros_like(s2), s2 * eb)
+    arg_n = torch.where(m2 > m, arg2, torch.where(m > m2, arg, torch.minimum(arg, arg2)))
+    return (torch.where(dead, m, mn), torch.where(dead, s, pa + pb), torch.where(dead, arg, arg_n))
+
+
+def decoder_f32_exact(acc, bias, targets, ex2, logf, mutant=None):
+    """The outputs of csrc/lm.cu bit for bit: acc [M, V] f32 the rows' accumulators of h W^T (the GEMM mainloop's
+    bits), bias [V] f32 or None, targets [M] (-100 ignored), ex2 / logf callables on f32 tensors (the device's through
+    ie_debug_gates, or ex2_rn / logf_rn).  Returns torch (nll f32, lse f32, pred int32) [M] on acc's device.
+
+    * logit = f32(acc + bias); columns >= V are -inf.
+    * Per row, 256-column tile n and quad lane q, the lane's 64 columns 256 n + 8 jg + 2 q + e in (jg, e) order: mx the
+      lane's max and am its first column; mn = max(m, mx); ts = the left-to-right f32 sum of exp_sub(x, mn); scale = 0
+      while m = -inf, else exp_sub(m, mn); s = fma(s, scale, ts); arg = am where mx > m; m = mn.  A lane whose columns
+      are all -inf skips the tile.  The tiles of a slice (32) run in order, the running maxima as a cummax.
+    * Per slice, the quad merges lanes (0, 1) and (2, 3), then the two results.
+    * The slices merge in order; lse = f32(m + logf(s)), nll = f32(lse - logit[y]) or 0 for y = -100; pred = arg.
+
+    ``mutant`` names an order the kernel must not have (negative controls, EXACT_MUTANTS): ``tiles_desc`` the tiles of
+    a slice in descending order, ``no_fma`` the rescale rounded twice, ``quad_pairs`` the quad merged as (0, 2), (1, 3),
+    ``slices_desc`` the slices combined in descending order, ``one_lane`` one 256-column chain per tile, ``log_f64``
+    lse = f32(m + log(s)) with the log and the add in float64."""
+    if mutant is not None and mutant not in EXACT_MUTANTS:
+        raise ValueError(f"unknown mutant {mutant!r}")
+    from .text_clas_ref import _f32, fma_f32
+    acc = torch.as_tensor(acc)
+    if acc.dtype != torch.float32 or acc.dim() != 2:
+        raise TypeError("acc must be a float32 [M, V] tensor")
+    dev = acc.device
+    M, V = acc.shape
+    ninf = -math.inf
+    b = torch.zeros(V, dtype=torch.float32, device=dev) if bias is None else \
+        torch.as_tensor(np.asarray(bias, np.float32)).to(dev)
+    t = torch.as_tensor(np.asarray(targets, np.int64)).to(dev)
+    if bool(((t != -100) & ((t < 0) | (t >= V))).any()):
+        raise ValueError("a target outside [0, V) other than -100")
+    logit = acc + b[None, :]
+    NT = -(-V // 256)
+    S = -(-NT // SLICE_TILES)
+    NTp = S * SLICE_TILES
+    x = torch.full((M, NTp * 256), ninf, dtype=torch.float32, device=dev)
+    x[:, :V] = logit
+    # lanes [M, tile, lane, k] and each entry's column inside its tile
+    if mutant == "one_lane":
+        lanes = x.view(M, NTp, 1, 256)
+        tcol = torch.arange(256, device=dev)[None, :]
+    else:
+        lanes = x.view(M, NTp, 32, 4, 2).permute(0, 1, 3, 2, 4).reshape(M, NTp, 4, 64)
+        jg, e = torch.arange(64, device=dev) // 2, torch.arange(64, device=dev) % 2
+        tcol = 8 * jg[None, :] + 2 * torch.arange(4, device=dev)[:, None] + e[None, :]
+    del x
+    Q, K = lanes.shape[2], lanes.shape[3]
+    tix = torch.arange(NTp, device=dev)                      # processing position -> tile
+    if mutant == "tiles_desc":
+        tix = tix.view(S, SLICE_TILES).flip(1).reshape(-1)
+        lanes = lanes[:, tix]
+    mx, kk = lanes.amax(dim=3), lanes.argmax(dim=3)          # argmax: the first maximal index, as `v > mx` keeps
+    am = (256 * tix[None, :, None] + tcol[torch.arange(Q, device=dev)[None, None, :], kk]).int()
+    mx, am = mx.view(M, S, SLICE_TILES, Q), am.view(M, S, SLICE_TILES, Q)
+    skip = mx == ninf
+    m_after = torch.cummax(mx, dim=2).values
+    m_prev = torch.cat([torch.full_like(m_after[:, :, :1], ninf), m_after[:, :, :-1]], 2)
+    mn = torch.where(skip, torch.zeros_like(m_after), m_after)   # skipped lanes: any finite value, masked below
+    terms = _exp_sub(lanes.view(M, S, SLICE_TILES, Q, K), mn[..., None], ex2)
+    del lanes
+    ts = terms[..., 0]
+    for k in range(1, K):
+        ts = ts + terms[..., k]
+    del terms
+    first = m_prev == ninf
+    scale = torch.where(first, torch.zeros_like(mn), _exp_sub(torch.where(first, mn, m_prev), mn, ex2))
+    s = torch.zeros(M, S, Q, dtype=torch.float64, device=dev)
+    for p in range(SLICE_TILES):
+        sc, tp = scale[:, :, p].double(), ts[:, :, p].double()
+        new = _f32(_f32(s * sc) + tp) if mutant == "no_fma" else fma_f32(s, sc, tp)
+        s = torch.where(skip[:, :, p], s, new)
+    s = s.float()
+    m = m_after[:, :, -1]
+    hit = (mx == m[:, :, None, :]) & ~skip
+    arg = am.gather(2, hit.to(torch.uint8).argmax(2, keepdim=True))[:, :, 0]
+    arg = torch.where(m == ninf, torch.full_like(arg, NO_ARG), arg)
+    lane = [(m[..., q], s[..., q], arg[..., q]) for q in range(Q)]
+    if Q == 1:
+        part = lane[0]
+    elif mutant == "quad_pairs":
+        part = _merge(_merge(lane[0], lane[2], ex2), _merge(lane[1], lane[3], ex2), ex2)
+    else:
+        part = _merge(_merge(lane[0], lane[1], ex2), _merge(lane[2], lane[3], ex2), ex2)
+    order = range(S - 1, -1, -1) if mutant == "slices_desc" else range(S)
+    tot = None
+    for k in order:
+        pk = tuple(v[:, k] for v in part)
+        tot = pk if tot is None else _merge(tot, pk, ex2)
+    m, s, arg = tot
+    if mutant == "log_f64":
+        lse = (m.double() + torch.log(s.double())).float()
+    else:
+        lse = m + logf(s)
+    zt = logit.gather(1, t.clamp_min(0)[:, None])[:, 0]
+    nll = torch.where(t == -100, torch.zeros_like(lse), lse - zt)
+    return nll, lse, arg.int()
 
 
 def check_decoder(ref: dict, nll, lse, pred) -> dict:

@@ -1,8 +1,11 @@
 """CPU tests of the language model's host side: the vectorised validation stream against a literal fastai
 LanguageModelPreLoader, the literal stateful validate loop against one zero-state run over whole rows, the state-dict
-refusals, the plain-C declarations and the ptxas figures of csrc/lm.cu."""
+refusals, the plain-C declarations and the ptxas figures of csrc/lm.cu; the exact float32 restatement of the decoder
+against the float64 bounds, its negative controls, and the SASS facts it rests on."""
+import functools
 import os
 import re
+import shutil
 import subprocess
 
 import numpy as np
@@ -129,3 +132,101 @@ def test_lm_cu_built_for_sm_90a():
     print("lm.cu ptxas spill stores:", figures)
     assert set(figures) == {"combine", "decode"}
     assert figures["combine"] == 0 and figures["decode"] <= 64
+
+
+# ------------------------------------------------------------------------------------------------ exact restatement
+def _int_case(E, V, M, seed):
+    rng = np.random.default_rng(seed)
+    h = rng.integers(-2, 3, size=(M, E)).astype(np.float32)
+    W = rng.integers(-3, 4, size=(V, E)).astype(np.float32)
+    b = rng.integers(-4, 5, size=V).astype(np.float32)
+    t = rng.integers(0, V, size=M)
+    t[0] = -100
+    t[-1] = V - 1
+    return h, W, b, t
+
+
+@pytest.mark.parametrize("E,V,M", [(7, 1, 3), (7, 257, 17), (16, 8193, 9), (16, 20000, 40)])
+def test_exact_restatement_within_the_f64_bounds(E, V, M):
+    """decoder_f32_exact with correctly rounded 2^x and log as stand-ins lies inside decoder_f64's per-element bounds
+    (small-integer h and W: the logits are exact, so the accumulators are h W^T in f32), and its argmax is the f64
+    argmax."""
+    h, W, b, t = _int_case(E, V, M, E + V + M)
+    acc = torch.from_numpy(h @ W.T)
+    nll, lse, pred = (v.numpy() for v in L.decoder_f32_exact(acc, b, t, L.ex2_rn, L.logf_rn))
+    ref = L.decoder_f64(h, W, b, t, 1)
+    v = L.check_decoder(ref, nll, lse, pred)
+    assert v["max_lse"] <= 1 and v["max_nll"] <= 1 and v["wrong_pred"] == 0, v
+    np.testing.assert_array_equal(pred, np.argmax(h.astype(np.float64) @ W.T.astype(np.float64) + b, 1))
+    assert nll[0] == 0
+
+
+def _mixed_acc(M, V, seed):
+    """Accumulators of two kinds: half the rows 4 N(0, 1) plus a bias, half a ramp (c - V) / 256 plus N(0, 1) that
+    rescales at every tile and ends near 0, where lse = log(s) shows the last bits of s."""
+    g = torch.Generator().manual_seed(seed)
+    acc = 4 * torch.randn(M, V, generator=g, dtype=torch.float64)
+    acc[M // 2:] = (torch.arange(V, dtype=torch.float64) - V) / 256 + torch.randn(M - M // 2, V, generator=g,
+                                                                                 dtype=torch.float64)
+    b = torch.randn(V, generator=g).float().numpy()
+    t = torch.randint(0, V, (M,), generator=g).numpy()
+    t[0] = -100
+    return acc.float(), b, t
+
+
+@functools.lru_cache(maxsize=1)
+def _mixed_case():
+    acc, b, t = _mixed_acc(96, 40000, 4)       # five slices
+    return acc, b, t, L.decoder_f32_exact(acc, b, t, L.ex2_rn, L.logf_rn)
+
+
+@pytest.mark.parametrize("mutant", L.EXACT_MUTANTS)
+def test_every_mutant_changes_output_bits(mutant):
+    acc, b, t, base = _mixed_case()
+    mut = L.decoder_f32_exact(acc, b, t, L.ex2_rn, L.logf_rn, mutant=mutant)
+    n = sum(int((x.view(torch.int32) != y.view(torch.int32)).sum()) for x, y in zip(base, mut))
+    assert n > 0, mutant
+
+
+def _sass_functions(obj):
+    """{function name: [(opcode, operands, line)]} of cuobjdump -sass, predicates dropped."""
+    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    if not os.path.exists(exe):
+        pytest.skip("cuobjdump is not installed")
+    text = subprocess.run([exe, "-sass", obj], capture_output=True, text=True, check=True).stdout
+    out = {}
+    for block in re.split(r"\n\s*Function : ", text)[1:]:
+        name = block.split("\n", 1)[0].strip()
+        out[name] = [(m.group(1), m.group(2).strip(), m.group(0)) for m in
+                     re.finditer(r"/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)\s*([^;]*);[^\n]*", block)]
+    return out
+
+
+def test_lm_sass_has_the_restated_order():
+    """The facts decoder_f32_exact rests on, read from build/lm.o: the decoder's GEMM instantiation has exactly two
+    FFMA (s = fma(s, scale, ts), one per row half); lm_combine_kernel has no FFMA but logf's own (the count in the
+    test kernel of ie_debug_gates fn 10 in build/misc.o, built with the same flags), so merge is two products and an
+    add; every MUFU.EX2 in both reads an FMUL by log2(e) as f32 (0x3fb8aa3b), i.e. ex2(f32(f32(x - m) * log2e)) with
+    nothing contracted into it."""
+    _lib.load()
+    build = os.path.join(ROOT, "code_intelligence_b200", "csrc", "build")
+    fns = _sass_functions(os.path.join(build, "lm.o"))
+    misc = _sass_functions(os.path.join(build, "misc.o"))
+    pick = lambda fs, key: [v for k, v in fs.items() if key in k]
+    decode, combine = pick(fns, "LmEpi"), pick(fns, "lm_combine_kernel")
+    logf = pick(misc, "debug_lm_math_kernelILi10E")
+    assert len(decode) == len(combine) == len(logf) == 1, list(fns)
+    decode, combine, logf = decode[0], combine[0], logf[0]
+    count = lambda ins, op: sum(1 for o, _, _ in ins if o == op)
+    assert count(decode, "FFMA") == 2, "the decoder's epilogue contracts other than s * scale + ts"
+    assert count(logf, "FFMA") > 0
+    assert count(combine, "FFMA") == count(logf, "FFMA"), "merge in lm_combine_kernel is contracted into an fma"
+    assert count(decode, "MUFU.EX2") >= 128 and count(combine, "MUFU.EX2") > 0
+    for name, ins in (("decode", decode), ("combine", combine)):
+        for i, (op, args, _) in enumerate(ins):
+            if op != "MUFU.EX2":
+                continue
+            src = args.split(",")[1].strip()
+            w = next((j for j in range(i - 1, -1, -1) if ins[j][1].split(",")[0].strip() == src), None)
+            assert w is not None and ins[w][0] == "FMUL" and "0x3fb8aa3b" in ins[w][2], \
+                (name, "MUFU.EX2 not fed by an FMUL by log2(e)", ins[i][2], None if w is None else ins[w][2])

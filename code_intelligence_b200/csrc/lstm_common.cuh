@@ -34,19 +34,23 @@ __device__ __forceinline__ float tanh_ieee(float x) {
 // One hidden unit of one batch row.  z* = the accumulator (h_{t-1} W_hh^T, plus x_t W_ih^T when the input projection
 // rides the K loop) + Gx (x_t W_ih^T + b_ih + b_hh) or the bias; gate order i, f, g, o as in torch.  The gate mode is a
 // template parameter so that an epilogue holds only the one gate path it runs.
+//
+// The contraction of c = f c_{t-1} + i g is spelled out in every gate mode: left to the compiler, the choice of which
+// product to fuse depends on the surrounding code, and outputs would change bits from one kernel to the next.  Each form
+// is the one the compiler had chosen for every kernel and the ie_debug_gates hook of its mode (measured on the H100 bit
+// for bit against oracle/device_numerics.teacher_forced_exact, DESIGN.md section 2): fast and exp gates round i g and
+// fuse f c_{t-1} onto it, the IEEE gates round f c_{t-1} and fuse i g onto it.  h = o tanh(c) is one rounded product.
 template <int GM>
 __device__ __forceinline__ void lstm_cell1(float zi, float zf, float zg, float zo, float cprev, float& cnew, float& hn) {
   if constexpr (GM == kGatesFast) {
-    cnew = sigmoid_fast(zf) * cprev + sigmoid_fast(zi) * tanh_fast(zg);
-    hn = sigmoid_fast(zo) * tanh_fast(cnew);
+    cnew = fmaf(sigmoid_fast(zf), cprev, __fmul_rn(sigmoid_fast(zi), tanh_fast(zg)));
+    hn = __fmul_rn(sigmoid_fast(zo), tanh_fast(cnew));
   } else if constexpr (GM == kGatesExp) {
-    cnew = sigmoid_acc(zf) * cprev + sigmoid_acc(zi) * tanh_acc(zg);
-    hn = sigmoid_acc(zo) * tanh_acc(cnew);
+    cnew = fmaf(sigmoid_acc(zf), cprev, __fmul_rn(sigmoid_acc(zi), tanh_acc(zg)));
+    hn = __fmul_rn(sigmoid_acc(zo), tanh_acc(cnew));
   } else {
-    // the contraction is spelled out: f c rounded, i g fused onto it (left to the compiler, the choice of which
-    // product to fuse depends on the surrounding code, and the fp32 mode's outputs would change bits)
     cnew = fmaf(sigmoid_ieee(zi), tanh_ieee(zg), __fmul_rn(sigmoid_ieee(zf), cprev));
-    hn = sigmoid_ieee(zo) * tanh_ieee(cnew);
+    hn = __fmul_rn(sigmoid_ieee(zo), tanh_ieee(cnew));
   }
 }
 

@@ -43,6 +43,9 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
+from oracle import tc_accum
+from oracle.text_clas_ref import fma_f32
+
 U24 = 2.0 ** -24                 # f32 unit roundoff
 TANH_APPROX_REL = 2.0 ** -10.9   # tanh.approx.f32: maximum relative error 2^-10.987 (PTX ISA)
 SPLIT_REL = 2.0 ** -16           # split-bf16 products vs the f32 operands, relative to sum |a b|
@@ -181,7 +184,8 @@ class Mode:
     Mutants: stale_c -- units that read c_{t-2} instead of c_{t-1} (a lost-ordering race); swap_fo -- units whose f and o
     gates are exchanged (a permutation slip).  Confined to one step (t, units): stale_c_at -- at step t the units read
     c_{t-2}; stale_h_at -- at step t the z of the units is formed from h_{t-2} (a ring slot read before it was written);
-    carry_lost_at = t0 -- at step t0 h_{t0-1} and c_{t0-1} read as zero (a lost time-chunk carry)."""
+    carry_lost_at = t0 -- at step t0 h_{t0-1} and c_{t0-1} read as zero (a lost time-chunk carry).
+    order: an order mutant of the exact restatement (teacher_forced_exact only, ORDER_MUTANTS)."""
     segs: int = 1
     gx: str = "fp16"
     gates: str = "fast"
@@ -191,6 +195,7 @@ class Mode:
     stale_c_at: tuple = ()
     stale_h_at: tuple = ()
     carry_lost_at: int = -1
+    order: str = ""
 
 
 EXACT = Mode(segs=0, gx="exact", gates="exact", cell="exact")
@@ -523,6 +528,196 @@ def mlp_head(X, coefs, intercepts, device=None):
         else:
             p, sl, sh = torch.sigmoid(z), torch.sigmoid(z - eps), torch.sigmoid(z + eps)
             return p, sl - sig_err(z - eps, sl, "exp"), sh + sig_err(z + eps, sh, "exp")
+
+
+# ------------------------------------------------------------------------------------------------ exact restatement
+# The same rounding points as above, but every operation between them restated exactly as the device performs it, so
+# that the device's outputs are predicted bit for bit: the MMA chain by tc_accum.chain_exact (tc_accum.MODEL, pinned on
+# the H100 by tests/test_gpu_primitives.py), f32 additions and products as float64 operations rounded once to f32
+# (correctly rounded: 53 >= 2 * 24 + 2 bits), fmas by text_clas_ref.fma_f32, and the gate functions by a caller-supplied
+# `gates(name, x)`: on the GPU the device's own inline functions through ie_debug_gates, elsewhere
+# the correctly rounded stand-in rounded_gates.  Every function takes and returns float64 torch tensors holding f32
+# (or narrower) values, on the device of its inputs.
+#
+# Order mutants (Mode.order, negative controls of the restatement): 'reversed' -- the k16 steps of every chain in
+# reverse; 'interleaved' -- split-bf16 passes hi*hi, lo*hi, hi*lo interleaved per 64-wide k-block instead of one pass
+# after the other; 'gx_init' -- Gx as the recurrent chain's starting value instead of added after it; 'bias_early' --
+# in the fused last layer the bias added between the W_ih and the W_hh part of the chain; 'cell_other' -- the other
+# contraction of the cell (CELL_FUSES_FC); 'gx_rz' -- the fp16 Gx store truncated toward zero.
+ORDER_MUTANTS = ("reversed", "interleaved", "gx_init", "bias_early", "cell_other", "gx_rz")
+GATE_FNS = {"fast": ("sigmoid_fast", "tanh_fast"), "exp": ("sigmoid_acc", "tanh_acc"),
+            "ieee": ("sigmoid_ieee", "tanh_ieee")}
+# the cell's contraction per gate kind (lstm_common.cuh lstm_cell1): True c = fma(f, c_{t-1}, f32(i g)), False
+# c = fma(i, g, f32(f c_{t-1}))
+CELL_FUSES_FC = {"fast": True, "exp": True, "ieee": False}
+
+
+def rounded_gates(name: str, x: torch.Tensor) -> torch.Tensor:
+    """Correctly rounded f32 sigmoid / tanh of f32 values: a stand-in for the device's gate function `name`."""
+    return rne_f32(torch.sigmoid(x) if name.startswith("sigmoid") else torch.tanh(x))
+
+
+def rz_fp16(x: torch.Tensor) -> torch.Tensor:
+    """Truncate toward zero to IEEE half (a mutant of the fp16 RNE store)."""
+    h = x.to(torch.float16)
+    up = h.to(x.dtype).abs() > x.abs()
+    return torch.where(up, torch.nextafter(h, torch.zeros_like(h)), h).to(x.dtype)
+
+
+def store(z: torch.Tensor, out_type: str) -> torch.Tensor:
+    """The epilogue's store of f32 values: f32, bf16 RNE, fp16 RNE (overflow to +-inf) or the mutant 'fp16_rz'."""
+    return {"f32": lambda v: v, "bf16": rne_bf16, "fp16": rne_fp16, "fp16_rz": rz_fp16}[out_type](z)
+
+
+def _pad16(x: torch.Tensor) -> torch.Tensor:
+    return torch.nn.functional.pad(x, (0, -x.shape[1] % 16))
+
+
+def order_pairs(pairs, order: str = ""):
+    """The operand pairs of a chain as an order mutant runs them ('reversed', 'interleaved'); unchanged otherwise."""
+    if order == "reversed":
+        return [(_pad16(x).flip(1), _pad16(w).flip(1)) for x, w in reversed(pairs)]
+    if order == "interleaved" and len(pairs) == 3:
+        pad64 = lambda v: torch.nn.functional.pad(v, (0, -v.shape[1] % 64))
+        xs, ws = [pad64(x) for x, _ in pairs], [pad64(w) for _, w in pairs]
+        blocks = range(0, xs[0].shape[1], 64)
+        return [(torch.cat([x[:, k:k + 64] for k in blocks for x in xs], 1),
+                 torch.cat([w[:, k:k + 64] for k in blocks for w in ws], 1))]
+    return pairs
+
+
+def gemm_exact(a, b, bias, act: int, out_type: str, segs: int, gates=rounded_gates, device=None, order: str = ""):
+    """act(a b^T + bias) as the library's GEMM stores it (gemm_kernel.cuh), bit for bit: the chain (split-bf16: the
+    three passes one after the other), f32(acc + bias), relu as fmaxf(x, 0), sigmoid as gates('sigmoid_acc', .) on the
+    f32 value, then the store of out_type ('f32' | 'bf16' | 'fp16').  a [M, K], b [N, K] f32 values, bias [N] or None.
+    Returns float64 [M, N]."""
+    a, b = _t(a, device), _t(b, device)
+    z = tc_accum.chain_exact(order_pairs(passes(operands(a, segs), operands(b, segs), segs), order))
+    if bias is not None:
+        z = rne_f32(z + rne_f32(_t(bias, a.device)))
+    if act == 1:
+        z = z.clamp_min(0)
+    elif act == 2:
+        z = gates("sigmoid_acc", z)
+    return store(z, out_type)
+
+
+def mlp_head_exact(X, coefs, intercepts, gates=rounded_gates, device=None):
+    """The MLP head as ie_mlp_predict_proba (api.cu) computes it, bit for bit: X f32 -> bf16, weights f32 -> bf16,
+    each hidden layer relu(acc + bias) stored as bf16, the last layer sigmoid_acc of the f32 acc + bias.
+    coefs [fan_in, fan_out] (sklearn layout), intercepts [fan_out].  Returns float64 [n, n_labels] (f32 values)."""
+    x = _t(np.asarray(X, dtype=np.float32), device)
+    n = len(coefs)
+    for l, (W, bvec) in enumerate(zip(coefs, intercepts)):
+        w = _t(np.asarray(W, dtype=np.float32), x.device).T
+        b = np.asarray(bvec, dtype=np.float32)
+        last = l == n - 1
+        x = gemm_exact(x, w, b, 2 if last else 1, "f32" if last else "bf16", 1, gates)
+    return x
+
+
+def teacher_forced_exact(x_in, h_dev, weights: dict, mode: Mode, rows=None, units=None, gates=rounded_gates,
+                         ids=None):
+    """Every h_t of one layer from the device's own inputs, bit for bit (teacher_forced_layer's prediction without an
+    error bound: nothing is left to bound).
+
+    x_in  [R, T, in] f32 values: the layer's input (the previous layer's device states); for layer 0 either the
+          embedding rows Emb[ids], or, with `ids` [R, T] given, the embedding matrix itself (Gx is then formed once per
+          distinct token, which gives the per-token table's bits and gather + GEMM's alike)
+    h_dev [R, T, out] this layer's device states: h_{t-1} is read from them as the ring holds it, bf16(h) or split
+    rows  the rows to predict (default all); units: the units to predict (default all).  h[:, :, u] needs only the four
+          gate columns of unit u, so restricting units shrinks every chain's N; K is never reduced.
+    Operands, Gx = store(f32(x W_ih^T + f32(b_ih + b_hh)), fp16 | f32) of its own chain, z = f32(acc + Gx) of the
+    recurrent chain (the fused last layer: one chain over x W_ih^T then h W_hh^T, z = f32(acc + bias)), the gate
+    functions on z, c = fma(f, c_{t-1}, f32(i g)) (fast, exp) or fma(i, g, f32(f c_{t-1})) (ieee) recursed exactly from
+    c = 0, h = f32(o tanh(c)).
+    Returns (h, c) float64 [len(rows), T, len(units)] on h_dev's device."""
+    if mode.segs not in (1, 3) or mode.gx not in ("fp16", "f32", "bf16", "fused") or mode.gates not in GATE_FNS:
+        raise ValueError(f"no exact restatement of {mode}")
+    pick = lambda v, r: v[r.to(v.device)] if isinstance(v, torch.Tensor) else np.asarray(v)[r.cpu().numpy()]
+    dev = h_dev.device if isinstance(h_dev, torch.Tensor) else torch.device("cpu")
+    H = h_dev.shape[2]
+    rows = torch.arange(h_dev.shape[0], device=dev) if rows is None else torch.as_tensor(rows, device=dev).long()
+    units = list(range(H)) if units is None else [int(u) for u in units]
+    U = len(units)
+    loc = {u: i for i, u in enumerate(units)}
+    hd = _t(pick(h_dev, rows), dev)
+    R, T = hd.shape[:2]
+    s, order = mode.segs, mode.order
+    cols = [q * H + u for q in range(4) for u in units]   # i, f, g, o of every unit, gate-major
+    w_ih, w_hh = _t(weights["w_ih"], dev)[cols], _t(weights["w_hh"], dev)[cols]
+    bias = _bias(weights, mode, dev)[cols]
+    if ids is None:
+        x_all = _t(pick(x_in, rows), dev)
+    else:
+        x_all = _t(x_in, dev)
+        ids = torch.as_tensor(np.asarray(ids.cpu() if isinstance(ids, torch.Tensor) else ids), device=dev)[rows]
+
+    def x_rows(sel_t=slice(None)):
+        """Layer inputs of the rows at steps sel_t -> ([n, in], index of each (row, t) into it or None)."""
+        if ids is None:
+            return x_all[:, sel_t].reshape(-1, x_all.shape[-1]), None
+        tok, inv = torch.unique(ids[:, sel_t].reshape(-1), return_inverse=True)
+        return x_all[tok], inv
+
+    def preact(hp, sel_t=slice(None)):
+        """z [n, 4U] of the (row, t) pairs at steps sel_t with h_{t-1} = hp [n, H]."""
+        h_pairs = passes(operands(hp, s), operands(w_hh, s), s)
+        x, inv = x_rows(sel_t)
+        if mode.gx == "fused":
+            if inv is not None:
+                x = x[inv]
+            x_pairs = passes(operands(x, s), operands(w_ih, s), s)
+            if order == "bias_early":
+                p0 = rne_f32(tc_accum.chain_exact(order_pairs(x_pairs)) + bias)
+                return tc_accum.chain_exact(h_pairs, p0)
+            return rne_f32(tc_accum.chain_exact(order_pairs(x_pairs + h_pairs, order)) + bias)
+        out = {"fp16": "fp16_rz" if order == "gx_rz" else "fp16", "f32": "f32", "bf16": "bf16"}[mode.gx]
+        gx = gemm_exact(x, w_ih, bias, 0, out, s, order=order if order in ("reversed", "interleaved") else "")
+        if inv is not None:
+            gx = gx[inv]
+        if order == "gx_init":
+            return tc_accum.chain_exact(h_pairs, gx)
+        return rne_f32(tc_accum.chain_exact(order_pairs(h_pairs, order)) + gx)
+
+    hprev = torch.cat([torch.zeros_like(hd[:, :1]), hd[:, :-1]], 1)
+    if mode.carry_lost_at >= 0:
+        hprev[:, mode.carry_lost_at] = 0
+    z = preact(hprev.reshape(R * T, H)).view(R, T, 4 * U)
+    if mode.stale_h_at:
+        t, mut = mode.stale_h_at
+        h2 = hd[:, t - 2] if t >= 2 else torch.zeros_like(hd[:, 0])
+        z2 = preact(h2, slice(t, t + 1))
+        mc = [q * U + loc[u] for q in range(4) for u in mut if u in loc]
+        z[:, t, mc] = z2[:, mc]
+    sig, tanh = GATE_FNS[mode.gates]
+    swap = tuple(loc[u] for u in mode.swap_fo if u in loc)
+    zi, zf, zg, zo = _gate_views(z, U, swap)
+    i, f, o = gates(sig, torch.stack([zi, zf, zo])).unbind(0)
+    g = gates(tanh, zg)
+    local = lambda us: [loc[u] for u in us if u in loc]
+    stale = local(mode.stale_c)
+    stale_at = (mode.stale_c_at[0], local(mode.stale_c_at[1])) if mode.stale_c_at else (-1, [])
+    c1 = torch.zeros(R, U, dtype=torch.float64, device=dev)
+    c2 = torch.zeros_like(c1)
+    cs = torch.empty(R, T, U, dtype=torch.float64, device=dev)
+    for t in range(T):
+        cp = c1
+        if stale or stale_at[0] == t:
+            cp = c1.clone()
+            sel = stale if stale_at[0] != t else sorted(set(stale) | set(stale_at[1]))
+            cp[:, sel] = c2[:, sel]
+        if mode.carry_lost_at == t:
+            cp = torch.zeros_like(c1)
+        if CELL_FUSES_FC[mode.gates] != (order == "cell_other"):
+            c = fma_f32(f[:, t], cp, rne_f32(i[:, t] * g[:, t]))
+        else:
+            c = fma_f32(i[:, t], g[:, t], rne_f32(f[:, t] * cp))
+        if mode.cell == "bf16":
+            c = rne_bf16(c)
+        cs[:, t] = c
+        c2, c1 = c1, c
+    return rne_f32(o * gates(tanh, cs)), cs
 
 
 # ------------------------------------------------------------------------------------------------ statistics

@@ -116,6 +116,22 @@ PROTOTYPES = {
     "ie_lm_launch_count": (C.c_int64, [C.c_void_p]),
     "ie_debug_lm_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),
+    "ie_gen_state_create": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),
+    "ie_gen_state_destroy": (None, [C.c_void_p]),
+    "ie_gen_state_reset": (C.c_int, [C.c_void_p]),
+    "ie_gen_topk": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                   C.c_void_p, C.c_int32, C.c_void_p]),
+    "ie_gen_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_double,
+                                     C.c_double, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "ie_gen_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
+    "ie_gen_beam_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                    C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                    C.c_void_p]),
+    "ie_gen_state_export": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "ie_debug_gen_topk": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                   C.c_int32]),
+    "ie_debug_gen_sample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_double, C.c_double,
+                                     C.c_void_p, C.c_void_p, C.c_int32]),
 }
 
 _lib = None

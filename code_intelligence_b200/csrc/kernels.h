@@ -67,7 +67,8 @@ struct LstmLayerArgs {
   const void* gx;          // f16 or f32 [rows, 4*out_pad] (bias folded in, fragment order): row t*b_pad + brow of the chunk, or token id
   const int* tok;          // optional time-major token ids of the whole call (per-token input-projection table)
   float* c;                // [b_pad, out_pad] cell state
-  __nv_bfloat16* y;        // ring (slot 0 = h before the chunk (zeros at t0 = 0); slot t+1 = h_t, t chunk-local)
+  int carry_c;             // 1: c holds c_{-1} of a carried state (global step 0 reads it); 0: c_{-1} = 0
+  __nv_bfloat16* y;        // ring (slot 0 = h before the chunk (zeros at t0 = 0 without a carried state); slot t+1 = h_t)
   float* raw;              // optional [raw_rows, T_total, raw_ld] f32 copy of h (get_raw_features)
   int raw_rows;            // rows of raw: the call's valid rows B (padding rows of the batch are not stored)
   float* pool_sum;         // optional [b_pad, out_pad] (last layer only; formats: lstm_common.cuh)
@@ -325,5 +326,27 @@ struct LmDecodeArgs {
 int lm_slices(int V);
 // logits = h W^T + bias, per valid row: lse, nll against its target and argmax; the logits are never stored
 cudaError_t launch_lm_decode(const LmDecodeArgs& a, cudaStream_t stream);
+
+// ---- text generation (lm_gen.cu): decisions on f32 logits [rows, ld] (columns < V) ------------------------------------
+constexpr int kLmTopkMax = 64;       // k of lm_topk
+constexpr int kLmBeamMax = 16384;    // rows * top_k candidates one CTA sorts in shared memory (fastai's defaults: 10000)
+// per row: values [rows, k] = the k largest f32(z - lse), descending, ties to the lower column; idx [rows, k] their
+// columns; column `exclude` (>= 0) counts in lse and is -inf among the values (fastai's no_unk)
+cudaError_t launch_lm_topk(const float* logits, long long ld, int rows, int V, int k, int exclude, float* values,
+                           int64_t* idx, cudaStream_t stream);
+// per row: one draw from fastai's predict weights (softmax, `exclude` zeroed, min_p > 0 masking, powf(p, inv_t)) at
+// the uniform u[row], never a column of weight 0: out[row] the column, flags[row] 1 when no column reached min_p (nothing masked), 2 when every
+// weight is 0 (err[0] |= 2, column 0)
+cudaError_t launch_lm_sample(const float* logits, long long ld, int rows, int V, const float* u, int exclude,
+                             float min_p, float inv_t, int64_t* out, int* flags, int* err, cudaStream_t stream);
+// the min(beam_sz, rows * top_k) lowest scores f32(parent_scores[r] - values[r, c]) in stable-sort order: their parent
+// rows, tokens (tokens[r, c]), scores, and nodes_out [n, L + 1] = nodes_in [rows, L] of the parent plus the token
+cudaError_t launch_lm_beam_select(const float* parent_scores, const float* values, const int64_t* tokens, int rows,
+                                  int top_k, int beam_sz, const int64_t* nodes_in, int L, int* parent, int64_t* token,
+                                  float* score, int64_t* nodes_out, cudaStream_t stream);
+// dst row i = src row parent[i] in each of `layers` layers (rows of row_bytes, layers layer_bytes apart, both multiples
+// of 16); a parent outside [0, src_rows) raises err[0] |= 4 and copies row 0
+cudaError_t launch_gather_rows(const void* src, void* dst, const int* parent, int n, int src_rows, long long row_bytes,
+                               long long layer_bytes, int layers, int* err, cudaStream_t stream);
 
 }  // namespace ie

@@ -97,6 +97,7 @@ struct KArgs {
   long long* diag;
   int T, t_begin, t0, T_total, ng, tiles, out_pad, nkb, segs, kh_pad, trace_items, fault, raw_rows;
   int pre_nkb;           // FUSE: k-blocks of the input projection that precede the recurrent ones in every item
+  int carry_c;           // 1: global step 0 reads c_{-1} from cstate (a carried state) instead of zero
 };
 
 // TOK: Gx rows are rows of the per-token input-projection table; GXBF: Gx / table stored as fp16 (f32 otherwise);
@@ -302,7 +303,7 @@ __device__ __forceinline__ void lstm_layer_body(const CUtensorMap& tm_h, const C
             const long long co = static_cast<long long>(brow0 + 8 * hr) * a.out_pad + unit0;
 #pragma unroll
             for (int s = 0; s < 4; ++s) {
-              cv[hr][s] = (tg == 0) ? make_float4(0.0f, 0.0f, 0.0f, 0.0f)
+              cv[hr][s] = (tg == 0 && !a.carry_c) ? make_float4(0.0f, 0.0f, 0.0f, 0.0f)
                                     : __ldcg(reinterpret_cast<const float4*>(a.cstate + co + 16 * s));
               if constexpr (FUSE && POOL)
                 mv[hr][s] = (tg == 0) ? make_float4(0.0f, 0.0f, 0.0f, 0.0f)
@@ -507,7 +508,7 @@ cudaError_t launch_layer_t(const LstmLayerArgs& a, int ctas, int tiles, cudaStre
   k.T = a.single_step ? 1 : a.T; k.t_begin = a.single_step ? a.t_step : 0;
   k.t0 = a.t0; k.T_total = a.T_total; k.ng = a.ng; k.tiles = tiles; k.out_pad = a.out_pad;
   k.nkb = a.kh_pad / 64; k.segs = a.segs; k.kh_pad = a.kh_pad;
-  k.trace_items = a.trace_items; k.fault = a.fault;
+  k.trace_items = a.trace_items; k.fault = a.fault; k.carry_c = a.carry_c;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(ctas);
   cfg.blockDim = dim3(kLThreads);

@@ -391,6 +391,52 @@ int64_t ie_lm_launch_count(const ie_lm* lm);
 int ie_debug_lm_decode(ie_lm* lm, const float* hs, const int64_t* targets, int32_t M, float* nll, float* lse,
                        int32_t* pred);
 
+/* Text generation: fastai LanguageLearner's predict and beam_search, one decision per call, from a recurrent state
+ * carried across calls.  A state handle borrows the LM (destroy it before the LM; destroying it first is fine) and
+ * holds `rows` rows (1 <= rows <= ie_encoder_max_batch) of every layer's h (as the encoder's ring holds it) and c (f32),
+ * zero after create and reset.  A step feeds ids [n, T] int64 (n <= rows) to rows 0..n-1 of the state, leaves their
+ * state after the last step there, and decides on the logits of that last step (the persistent GEMM on the ring, f32).
+ * Host pointers: synchronous; device errors are returned.  IE_FLAG_DEVICE_PTRS: asynchronous on `stream`, outputs stay
+ * on the device (a step's token ids can be the next step's ids); ie_lm_check_errors() reports IE_ERR_TOKEN for an id
+ * outside [0, vocab_sz), and IE_ERR_INVALID for a sampled row of zero weight or a select index out of range.  Each
+ * call clears the error words of the call before it: collect them after every device-pointer call whose errors matter
+ * (or read `draw_flags`, which keep each row's outcome).  Argument errors return IE_ERR_INVALID before anything is
+ * launched. */
+typedef struct ie_gen_state ie_gen_state;
+int ie_gen_state_create(ie_lm* lm, int32_t rows, ie_gen_state** out);
+void ie_gen_state_destroy(ie_gen_state* st);
+int ie_gen_state_reset(ie_gen_state* st);
+/* Top k (1 <= k <= min(64, vocab_sz)) of each row's log_softmax at the last step: values [n, k] f32 descending, idx
+ * [n, k] int64, ties to the lower id.  exclude in [-1, vocab_sz): that id (fastai's no_unk) counts in the softmax's sum
+ * and is -inf among the values; -1 none. */
+int ie_gen_topk(ie_gen_state* st, const int64_t* ids, int32_t n, int32_t T, int32_t k, int32_t exclude,
+                     float* values, int64_t* idx, int32_t flags, void* stream);
+/* One id per row drawn from fastai's predict weights at the last step: p = softmax, p[exclude] = 0, with min_p in (0, 1]
+ * (0: none) p < min_p zeroed unless no p >= min_p, then p ** (1 / temperature) (temperature > 0): the first id of
+ * positive weight whose running sum exceeds u[r] * sum (u[r] in [0, 1), n floats); an id of weight 0 is never drawn.
+ * idx [n] int64; draw_flags [n] int32: 1 when no p reached min_p (nothing was masked), 2 when every weight was 0 (id 0
+ * is written and the call is in error: there is nothing to draw from). */
+int ie_gen_sample(ie_gen_state* st, const int64_t* ids, int32_t n, int32_t T, const float* u, int32_t exclude,
+                       double temperature, double min_p, int64_t* idx, int32_t* draw_flags, int32_t flags,
+                       void* stream);
+/* fastai's select_hidden: rows 0..n-1 of the state become its rows parent[0..n-1] (int32 in [0, rows)), n <= rows. */
+int ie_gen_select(ie_gen_state* st, const int32_t* parent, int32_t n, int32_t flags, void* stream);
+/* One beam step: candidate j = r * top_k + c (rows * top_k <= 16384) scores f32(scores[r] - values[r, c]); the
+ * m = min(beam_sz, rows * top_k) lowest in the order of a stable sort survive: parent [m] int32 (j / top_k), token [m]
+ * int64 (tokens[r, c]), new_scores [m] f32, new_nodes [m, L + 1] int64 = nodes [rows, L] of the parent (NULL when
+ * L = 0) followed by the token.  Does not touch the state: select(parent) follows. */
+int ie_gen_beam_select(ie_gen_state* st, const float* scores, const float* values, const int64_t* tokens, int32_t rows,
+                      int32_t top_k, int32_t beam_sz, const int64_t* nodes, int32_t L, int32_t* parent, int64_t* token,
+                      float* new_scores, int64_t* new_nodes, int32_t flags, void* stream);
+/* Test hook: rows 0..n-1 of the state's `layer`: h [n, P * out_l] uint16 (bf16 bits; P = 2 planes [hi | lo] with
+ * IE_CFG_FP32, else 1) and c [n, out_l] f32 (host).  Waits for the last call. */
+int ie_gen_state_export(ie_gen_state* st, int32_t layer, int32_t n, uint16_t* h, float* c);
+/* Test hooks: the top-k and sampling kernels on host logits [rows, V] f32 (same arguments as above). */
+int ie_debug_gen_topk(const float* logits, int32_t rows, int32_t V, int32_t k, int32_t exclude, float* values,
+                     int64_t* idx, int32_t device);
+int ie_debug_gen_sample(const float* logits, int32_t rows, int32_t V, const float* u, int32_t exclude,
+                       double temperature, double min_p, int64_t* idx, int32_t* draw_flags, int32_t device);
+
 #ifdef __cplusplus
 }
 #endif

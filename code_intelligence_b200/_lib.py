@@ -188,13 +188,14 @@ def _debug_gemm(a, b, bias=None, act: int = 0, out_type: int = 0, segs: int = 1,
 
 GATE_FNS = ("sigmoid_fast", "tanh_fast", "sigmoid_acc", "tanh_acc", "sigmoid_ieee", "tanh_ieee")
 CELL_FNS = {"fast": 6, "exp": 7, "ieee": 8}
-LM_MATH_FNS = {"lm_ex2": 9, "lm_log": 10}   # the language-model decoder's ex2.approx.ftz and logf (csrc/lm.cu)
+# the language-model decoder's ex2.approx.ftz and logf (csrc/lm.cu), text generation's expf (csrc/lm_gen.cu)
+LM_MATH_FNS = {"lm_ex2": 9, "lm_log": 10, "lm_expf": 11}
 
 
 def _debug_gates(fn, x):
     """Test hook ``ie_debug_gates`` on CUDA float32 tensors.  fn a name of GATE_FNS or LM_MATH_FNS: f(x) elementwise,
-    same shape.  fn 'cell_fast' | 'cell_exp' | 'cell_ieee': x [5, n] planes (zi, zf, zg, zo, c_prev) -> [2, n]
-    (c_new, h)."""
+    same shape.  fn 'lm_pow' (text generation's powf): x [2, n] planes (x, y) -> [n] powf(x, y).  fn 'cell_fast' |
+    'cell_exp' | 'cell_ieee': x [5, n] planes (zi, zf, zg, zo, c_prev) -> [2, n] (c_new, h)."""
     import torch
     x = x.contiguous()
     if x.dtype != torch.float32 or not x.is_cuda:
@@ -202,6 +203,11 @@ def _debug_gates(fn, x):
     if fn in GATE_FNS or fn in LM_MATH_FNS:
         code = GATE_FNS.index(fn) if fn in GATE_FNS else LM_MATH_FNS[fn]
         n, out = x.numel(), torch.empty_like(x)
+    elif fn == "lm_pow":
+        if x.dim() != 2 or x.shape[0] != 2:
+            raise ValueError(f"powf input {tuple(x.shape)} must be [2, n]")
+        code, n = 12, x.shape[1]
+        out = torch.empty(n, dtype=torch.float32, device=x.device)
     else:
         code = CELL_FNS[fn.removeprefix("cell_")]
         if x.dim() != 2 or x.shape[0] != 5:

@@ -1200,7 +1200,7 @@ int ie_debug_gemm(const float* a, const float* b, const float* bias, int32_t M, 
 }
 
 int ie_debug_gates(int32_t fn, const float* in, float* out, int64_t n, int32_t device, void* stream) {
-  if (in == nullptr || out == nullptr || n < 0 || fn < 0 || fn > 10)
+  if (in == nullptr || out == nullptr || n < 0 || fn < 0 || fn > 12)
     return fail(IE_ERR_INVALID, "fn=%d n=%lld: bad argument", fn, static_cast<long long>(n));
   CK(cudaSetDevice(device));
   CK(ie::launch_debug_gates(fn, in, out, n, static_cast<cudaStream_t>(stream)));

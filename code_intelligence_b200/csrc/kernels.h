@@ -117,7 +117,7 @@ cudaError_t launch_convert_rows(const float* src, long long ld_src, int cols, co
                                 __nv_bfloat16* dst, long long ld_dst, int lo_off, cudaStream_t stream);
 cudaError_t launch_fill_f32(float* p, size_t n, float v, cudaStream_t stream);
 // ie_debug_gates: fn 0..5 unary gate functions, 6 / 7 / 8 the cell update with fast / exp / IEEE gates, 9 / 10 the
-// language-model decoder's ex2_approx and logf
+// language-model decoder's ex2_approx and logf, 11 / 12 text generation's expf and powf (in = planes [x | y])
 cudaError_t launch_debug_gates(int fn, const float* in, float* out, long long n, cudaStream_t stream);
 
 // ---- precision-recall threshold search (pr_curve.cu): scores [n, n_labels] f32, truth [n, n_labels] u8 (device) ----------

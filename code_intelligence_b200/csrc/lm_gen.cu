@@ -9,11 +9,17 @@
 //
 // Every sum runs in one fixed order that does not depend on the grid, so a row's result is a function of its own logits:
 //   * column sums (the softmax denominator): thread t of the CTA adds columns t, t + kGenThreads, ... in ascending
-//     order, then the kGenThreads partials are reduced by xor shuffles (offsets 16, 8, 4, 2, 1) within each warp and
-//     the 32 warp sums are added in warp order by warp 0 the same way;
+//     order (the compiler fuses expf's final scale multiply into the add: s = fma(2^i, ex2(r), s)), then the
+//     kGenThreads partials are reduced by xor shuffles (offsets 16, 8, 4, 2, 1) within each warp and the 32 warp sums
+//     are added in warp order by warp 0 the same way;
 //   * the sampling CDF: columns in chunks of kGenThreads in ascending order; a chunk's inclusive prefix is a warp scan
 //     (Hillis-Steele, offsets 1 .. 16) plus the exclusive sum of the earlier warps' totals, itself a warp scan; the
-//     running total S_j = carry + prefix is rounded once per element, and the carry moves by the chunk's last S_j.
+//     running total S_j = carry + prefix is rounded once per element.  The carry then moves by the chunk's total as
+//     the scan of the warp totals has it at lane 31 (red[31]).  That is not the chunk's last S_j: thread 1023's prefix
+//     adds its warp's own prefix to red[30], another association, and on random weights the two differ in the last
+//     bit in about half of all chunks.  The row's total is the final carry, so it is not S_{V-1} either, even for
+//     V <= kGenThreads.
+//   oracle/lm_gen_ref.py restates both kernels bit for bit in this order.
 #include <climits>
 #include <cstdint>
 
@@ -201,9 +207,9 @@ __global__ void __launch_bounds__(kGenThreads) lm_topk_kernel(const float* __res
 //   w_j = 0 at the excluded column; with min_p > 0, 0 where p_j < min_p unless no column has p_j >= min_p (then
 //   flags[r] = 1 and nothing is masked); with inv_t != 1, w_j = powf(w_j, inv_t);
 // and the draw: the first column j of positive weight whose running sum S_j (fixed order, file comment) exceeds
-// f32(u_r * S_{V-1}).  The scan is not monotone in rounding (a lane's prefix sums its terms in another order than its
-// left neighbour's, so a zero weight can round one ulp above the column before it): columns of weight 0 are skipped
-// explicitly and can never be drawn.  When no positive column's S_j exceeds the target (it rounded up to the total),
+// f32(u_r * total), total the final carry of the scan (the file comment: not S_{V-1}).  The scan is not monotone in
+// rounding (a lane's prefix sums its terms in another order than its left neighbour's, so a zero weight can round one
+// ulp above the column before it): columns of weight 0 are skipped explicitly and can never be drawn.  When no positive column's S_j exceeds the target (it rounded up to the total),
 // the last column of positive weight is drawn.  A total of 0 sets flags[r] = 2 and bit 1 of err and draws column 0.
 __global__ void __launch_bounds__(kGenThreads) lm_sample_kernel(const float* __restrict__ logits, long long ld, int V,
                                                                  const float* __restrict__ u, int exclude, float min_p,
@@ -231,7 +237,7 @@ __global__ void __launch_bounds__(kGenThreads) lm_sample_kernel(const float* __r
     if (mask_min && p < min_p) return 0.0f;
     return inv_t != 1.0f ? powf(p, inv_t) : p;
   };
-  // pass 1: the total S_{V-1} and the last column of positive weight; pass 2: the first S_j above the target
+  // pass 1: the total (the final carry) and the last column of positive weight; pass 2: the first S_j above the target
   if (tid == 0) { found = INT_MAX; last_pos = -1; }
   __syncthreads();
   float carry = 0.0f, chunk_total;
@@ -239,7 +245,7 @@ __global__ void __launch_bounds__(kGenThreads) lm_sample_kernel(const float* __r
     const float wv = weight(base + tid);
     if (wv > 0.0f) atomicMax(&last_pos, base + tid);
     block_scan(wv, red, &chunk_total);
-    carry = carry + chunk_total;   // = the chunk's last S_j
+    carry = carry + chunk_total;   // red[31], not the chunk's last S_j (file comment)
   }
   const float total = carry;
   const float target = u[blockIdx.x] * total;

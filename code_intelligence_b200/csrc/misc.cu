@@ -187,14 +187,19 @@ __global__ void debug_gate_kernel(const float* __restrict__ x, float* __restrict
 }
 
 // the language-model decoder's 2^x (FN 9) and log (FN 10), inlined as lm.cu inlines them: ex2_approx (ptx.cuh) and
-// logf under lm.cu's compiler flags.  One copy of the function per kernel, so that the SASS of FN 10 is logf's alone
-// and can be compared with lm_combine_kernel's.
+// logf under lm.cu's compiler flags; text generation's expf (FN 11) and powf(x, y) (FN 12, in = planes [x | y]) under
+// lm_gen.cu's (the same flags).  One copy of the function per kernel, so that the SASS of FN 10 is logf's alone and
+// can be compared with lm_combine_kernel's and lm_topk_kernel's, and FN 11's expf ends in its own rounded multiply.
 template <int FN>
 __global__ void debug_lm_math_kernel(const float* __restrict__ x, float* __restrict__ y, long long n) {
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
 #pragma unroll 1
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
-    y[i] = FN == 9 ? ex2_approx(x[i]) : logf(x[i]);
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if constexpr (FN == 9) y[i] = ex2_approx(x[i]);
+    else if constexpr (FN == 10) y[i] = logf(x[i]);
+    else if constexpr (FN == 11) y[i] = expf(x[i]);
+    else y[i] = powf(x[i], x[n + i]);
+  }
 }
 
 // in = planes [zi | zf | zg | zo | c_prev] of n values, out = planes [c_new | h]
@@ -282,6 +287,8 @@ cudaError_t launch_debug_gates(int fn, const float* in, float* out, long long n,
     case 8: debug_cell_kernel<kGatesIeee><<<g, 256, 0, stream>>>(in, out, n); break;
     case 9: debug_lm_math_kernel<9><<<g, 256, 0, stream>>>(in, out, n); break;
     case 10: debug_lm_math_kernel<10><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 11: debug_lm_math_kernel<11><<<g, 256, 0, stream>>>(in, out, n); break;
+    case 12: debug_lm_math_kernel<12><<<g, 256, 0, stream>>>(in, out, n); break;
     default: return cudaErrorInvalidValue;
   }
   return cudaGetLastError();

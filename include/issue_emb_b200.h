@@ -193,12 +193,14 @@ int ie_debug_gemm_frag(const float* a, const float* b, const float* bias, int32_
 int64_t ie_debug_epilogue_layout(int32_t out_units, int32_t* perm, int64_t cap, int32_t* frag2, int32_t* frag4);
 
 /* Debug / test hook, device pointers on `device`, asynchronous on `stream`: the gate functions and the cell update as the
- * recurrent kernel and the GEMM epilogue compute them, and the language-model decoder's two math functions (the same
- * inline device functions).
+ * recurrent kernel and the GEMM epilogue compute them, and the language model's math functions (the same inline device
+ * functions, under the same compiler flags).
  *   fn 0..5: out[i] = f(in[i]), i < n, f = sigmoid_fast, tanh_fast, sigmoid_acc, tanh_acc, sigmoid_ieee, tanh_ieee
  *   fn 6, 7, 8: the cell update with fast, exp (IE_CFG_ACCURATE_GATES) or IEEE (IE_CFG_FP32) gates:
  *   in = planes [zi | zf | zg | zo | c_prev] of n values each, out = planes [c_new | h]
- *   fn 9, 10: out[i] = f(in[i]), f = the decoder's 2^x (ex2.approx.ftz.f32) and its logf. */
+ *   fn 9, 10: out[i] = f(in[i]), f = the decoder's 2^x (ex2.approx.ftz.f32) and its logf
+ *   fn 11: out[i] = expf(in[i]), text generation's expf
+ *   fn 12: out[i] = powf(in[i], in[n + i]): in = planes [x | y] of n values each, text generation's powf */
 int ie_debug_gates(int32_t fn, const float* in, float* out, int64_t n, int32_t device, void* stream);
 
 /* Debug / test hook: the hidden states of layer `layer` of an encode of ids [B, T] (zero initial state), as that

@@ -332,26 +332,36 @@ def test_all_zero_weights_are_reported():
 
 
 # ------------------------------------------------------------------------------------------------ beam selection
-@pytest.mark.parametrize("rows,top_k", [(1, 1), (10, 10), (1000, 10), (256, 64)])
+@pytest.mark.parametrize("rows,top_k", [(1, 1), (10, 10), (1000, 10), (256, 64), (3, 1), (1025, 1), (5461, 3)])
 def test_beam_select_is_a_stable_argsort(rows, top_k):
+    """n = rows * top_k candidates from 1 to 16383 (3, 1025 and 16383 pad the bitonic sort, and the padding keys must
+    sort last), beam_sz 1, n, n + 1 and 1000, nodes of L = 3 and L = 0 columns; -0 parent scores (-0 - 0 = -0, which
+    sorts as +0 and comes back as +0) and a -inf value (a +inf score) among the ties."""
     ref = L.make_lm(seed=1, vocab_sz=300, emb_sz=64, n_hid=64, n_layers=2)
     lm = device_lm(ref, 0)
     st = lm.new_state(1)
     try:
         rng = np.random.default_rng(rows * top_k)
         scores = rng.integers(0, 4, rows).astype(np.float32) * 0.5
-        values = -rng.integers(0, 6, (rows, top_k)).astype(np.float32) * 0.25   # many ties
+        scores[scores == 0] = -0.0
+        values = -rng.integers(0, 6, (rows, top_k)).astype(np.float32) * 0.25 + np.float32(0)   # many ties, +0
         values[0, 0] = -np.inf if rows * top_k > 1 else values[0, 0]
         tokens = rng.integers(0, 60000, (rows, top_k))
-        nodes = rng.integers(0, 60000, (rows, 3))
-        beam_sz = 1000
-        parent, token, sc, nn = lm.beam_select(st, scores, values, tokens, beam_sz, nodes)
-        cand = (scores[:, None] - values).reshape(-1).astype(np.float32)
-        order = np.argsort(cand, kind="stable")[:beam_sz]
-        np.testing.assert_array_equal(parent, order // top_k)
-        np.testing.assert_array_equal(token, tokens.reshape(-1)[order])
-        np.testing.assert_array_equal(sc, cand[order])
-        np.testing.assert_array_equal(nn, np.concatenate([nodes[order // top_k], tokens.reshape(-1)[order][:, None]], 1))
+        n = rows * top_k
+        for L_ in (3, 0):
+            nodes = rng.integers(0, 60000, (rows, L_))
+            for beam_sz in sorted({1, n, n + 1, 1000}):
+                parent, token, sc, nn = lm.beam_select(st, scores, values, tokens, beam_sz, nodes if L_ else None)
+                cand = (scores[:, None] - values).reshape(-1).astype(np.float32)
+                order = np.argsort(cand, kind="stable")[:beam_sz]
+                what = f"n={n} beam_sz={beam_sz} L={L_}"
+                np.testing.assert_array_equal(parent, order // top_k, err_msg=what)
+                np.testing.assert_array_equal(token, tokens.reshape(-1)[order], err_msg=what)
+                np.testing.assert_array_equal(sc.view(np.int32), (cand[order] + np.float32(0)).view(np.int32),
+                                              err_msg=what)
+                np.testing.assert_array_equal(nn, np.concatenate([nodes[order // top_k],
+                                                                  tokens.reshape(-1)[order][:, None]], 1), err_msg=what)
+        assert n < 1000 or np.any(np.isposinf(cand)) and np.any(np.signbit(cand) & (cand == 0))
     finally:
         st.close()
         lm.close()

@@ -5,7 +5,6 @@ against the float64 bounds, its negative controls, and the SASS facts it rests o
 import functools
 import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -16,6 +15,7 @@ from code_intelligence_b200 import _lib
 from code_intelligence_b200 import language_model as LM
 from oracle import awd_lstm_ref as R
 from oracle import lm_ref as L
+from oracle.sass import sass_functions
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -188,20 +188,6 @@ def test_every_mutant_changes_output_bits(mutant):
     assert n > 0, mutant
 
 
-def _sass_functions(obj):
-    """{function name: [(opcode, operands, line)]} of cuobjdump -sass, predicates dropped."""
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(exe):
-        pytest.skip("cuobjdump is not installed")
-    text = subprocess.run([exe, "-sass", obj], capture_output=True, text=True, check=True).stdout
-    out = {}
-    for block in re.split(r"\n\s*Function : ", text)[1:]:
-        name = block.split("\n", 1)[0].strip()
-        out[name] = [(m.group(1), m.group(2).strip(), m.group(0)) for m in
-                     re.finditer(r"/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)\s*([^;]*);[^\n]*", block)]
-    return out
-
-
 def test_lm_sass_has_the_restated_order():
     """The facts decoder_f32_exact rests on, read from build/lm.o: the decoder's GEMM instantiation has exactly two
     FFMA (s = fma(s, scale, ts), one per row half); lm_combine_kernel has no FFMA but logf's own (the count in the
@@ -210,8 +196,8 @@ def test_lm_sass_has_the_restated_order():
     nothing contracted into it."""
     _lib.load()
     build = os.path.join(ROOT, "code_intelligence_b200", "csrc", "build")
-    fns = _sass_functions(os.path.join(build, "lm.o"))
-    misc = _sass_functions(os.path.join(build, "misc.o"))
+    fns = sass_functions(os.path.join(build, "lm.o"))
+    misc = sass_functions(os.path.join(build, "misc.o"))
     pick = lambda fs, key: [v for k, v in fs.items() if key in k]
     decode, combine = pick(fns, "LmEpi"), pick(fns, "lm_combine_kernel")
     logf = pick(misc, "debug_lm_math_kernelILi10E")

@@ -1,4 +1,4 @@
-// Internal launch interfaces between the C-ABI layer (api.cu) and the sm_90a kernels.
+// Internal launch interfaces between the C-ABI layer (api_*.cu) and the sm_90a kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -55,7 +55,7 @@ cudaError_t launch_gemm_bf16(const GemmArgs& g, cudaStream_t stream);
 constexpr int kMaxBatches = 12;
 struct LstmLayerArgs {
   CUtensorMap tm_h;        // hidden-state ring of the time chunk [(Tc+1)*b_pad rows, ring cols], box {64, 128}
-  CUtensorMap tm_w;        // W_hh [4*out_pad rows, cols], box {64, 256}; rows ordered as api.cu slice_perm
+  CUtensorMap tm_w;        // W_hh [4*out_pad rows, cols], box {64, 256}; rows ordered as api_encoder.cu slice_perm
   CUtensorMap tm_h64;      // same tensor as tm_h with box {64, 64}: the half tile one CTA multicasts (mc != 0)
   CUtensorMap tm_x;        // pre_nkb > 0: the PREVIOUS layer's ring (slot t+1 = this layer's x_t), box {64, 128}
   int pre_nkb;             // > 0: fuse the input projection into the K loop -- pre_nkb = kin_pad / 64 k-blocks of

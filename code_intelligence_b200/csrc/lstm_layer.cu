@@ -7,7 +7,7 @@
 //
 // Work decomposition ("rotating schedule"):
 //   * an ITEM is 128 batch rows x one column tile of 256 accumulator columns = 64 hidden units x (i,f,g,o).  Weight rows
-//     are pre-permuted (api.cu slice_perm) so that the wgmma fragment of a thread holds all four gates of a unit: inside
+//     are pre-permuted (api_encoder.cu slice_perm) so that the wgmma fragment of a thread holds all four gates of a unit: inside
 //     16-column chunk m = 4s + e, columns 2q, 2q+1 are (i, f) and 8+2q, 9+2q are (g, o) of unit 16s + 4q + e -- the cell
 //     update needs no cross-thread traffic, and a thread's units come in runs of four (16-byte c, 8-byte h accesses);
 //     Gx is stored in the matching fragment order (kernels.h frag_index): 16-byte loads;

@@ -76,7 +76,7 @@ __global__ void embed_gather_kernel(const int64_t* __restrict__ ids, int B, int 
 
 // ids [B, T] int64 (batch-first) -> tok [T * b_pad] int32 (time-major, rows b >= B get the pad token), with the same
 // range check as embed_gather_kernel.  Used when layer 0 reads its input projection from the per-token table
-// (api.cu: IE_EMB_PROJ) instead of a GEMM over gathered embedding rows.
+// (api_encoder.cu: IE_EMB_PROJ) instead of a GEMM over gathered embedding rows.
 __global__ void tokens_time_major_kernel(const int64_t* __restrict__ ids, int B, int T, int b_pad, int vocab, int pad_idx,
                                          int* __restrict__ tok, int* err_flag) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;

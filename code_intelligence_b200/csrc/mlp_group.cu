@@ -1,5 +1,5 @@
 // Grouped training of the label MLP: the stages of mlp_train.cu and the persistent GEMM (gemm_kernel.cuh), each run
-// once for every model of a group that shares a step's shape.  api.cu's ie_mlp_group_* sequence launches them.
+// once for every model of a group that shares a step's shape.  api_mlp_train.cu's ie_mlp_group_* sequence launches them.
 //
 // Model j of a launch is slot slots[j] of the group; its operands sit at base + slot * stride.  Each kernel performs,
 // for every model, exactly the arithmetic of its single-model counterpart in mlp_train.cu over the same partition of

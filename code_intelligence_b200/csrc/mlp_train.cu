@@ -1,5 +1,5 @@
 // Training step of the label MLP (sklearn MLPClassifier, solver 'adam', relu hidden layers, logistic output): the
-// elementwise stages around the persistent GEMM (gemm.cu) that api.cu's ie_mlp_train_* sequence launches.
+// elementwise stages around the persistent GEMM (gemm.cu) that api_mlp_train.cu's ie_mlp_train_* sequence launches.
 //
 //   split_store_kernel   f32 [rows, cols] (optional row gather, optional relu mask) -> split-bf16 operands: row-major
 //                        [hi | lo] for the next product's A, transposed [hi | lo] (K = batch) for a weight gradient, and
@@ -11,7 +11,7 @@
 //
 // Every reduction runs in a fixed order without atomics, so a fit is deterministic.
 //
-// mlp_group.cu repeats each of these kernels for many models at once, and api.cu's mg_* sequence repeats mt_forward /
+// mlp_group.cu repeats each of these kernels for many models at once, and api_mlp_train.cu's mg_* sequence repeats mt_forward /
 // mt_backward / mt_adam; a grouped fit is bit-identical to a single one only while each pair does the same arithmetic
 // over the same partition, so change both together (tests/test_gpu_mlp_grid_search.py checks the pairs bit for bit).
 #include <cuda_bf16.h>

@@ -6,7 +6,7 @@ with the kernel line that performs it (paths relative to code_intelligence_b200/
   operands       bf16 RNE of the embedding, the weights and the layer inputs      misc.cu convert_rows_kernel
                  split-bf16 in the fp32-accurate mode: hi = bf16(x), lo = bf16(x - hi),
                  products hi*hi + lo*hi + hi*lo (the lo*lo term is dropped)        gemm.cu / lstm_layer.cu K loops
-  bias           f32(b_ih + b_hh), summed on the host in f32                       api.cu ie_encoder_load_layer
+  bias           f32(b_ih + b_hh), summed on the host in f32               api_encoder.cu ie_encoder_load_layer
   Gx             fp16 RNE of f32(x W_ih^T + bias): the layer-0 per-token table and
                  the middle layers' input projections                              gemm.cu pack_f16x2 (epilogue store)
                  f32 with IE_GX_BF16=0 / IE_CFG_F32_GX / IE_CFG_FP32
@@ -19,7 +19,7 @@ with the kernel line that performs it (paths relative to code_intelligence_b200/
                  max and last exact                                                lstm_common.cuh pool_accumulate1,
                                                                                    misc.cu pool_finalize_kernel
   MLP head       bf16 X and weights, f32 accumulate + bias, relu, bf16 hidden store,
-                 sigmoid_acc on the f32 output                                     api.cu ie_mlp_predict_proba, gemm.cu
+                 sigmoid_acc on the f32 output                                 api_mlp.cu ie_mlp_predict_proba, gemm.cu
 
 Teacher forcing.  A free-running reference cannot separate these rounding points from each other: rounding flips of the
 bf16 ring carry forward through the recurrence, and their effect is as large as the effect of a wrong rounding point.
@@ -203,7 +203,7 @@ EXACT = Mode(segs=0, gx="exact", gates="exact", cell="exact")
 
 def layer_modes(n_layers: int, flags: int = 0, env: dict | None = None):
     """The Mode of every layer for an encoder created with `flags` under the development knobs `env`, as
-    api.cu ie_encoder_create / run_encoder choose them (assumes the persistent grid is co-resident)."""
+    api_encoder.cu ie_encoder_create / run_encoder choose them (assumes the persistent grid is co-resident)."""
     env = {k: str(v) for k, v in (env or {}).items()}
     if flags & IE_CFG_FP32:
         segs, gx, gates = 3, "f32", "ieee"
@@ -228,7 +228,7 @@ def _bias(w, mode: Mode, device):
     b_ih, b_hh = np.asarray(w["b_ih"]), np.asarray(w["b_hh"])
     if mode.gx == "exact":
         return _t(b_ih.astype(np.float64) + b_hh.astype(np.float64), device)
-    return _t(b_ih.astype(np.float32) + b_hh.astype(np.float32), device)   # api.cu: f32 sum on the host
+    return _t(b_ih.astype(np.float32) + b_hh.astype(np.float32), device)   # api_encoder.cu: f32 sum on the host
 
 
 def _preactivation(px, ex, ph, eh, bias, mode: Mode):
@@ -508,7 +508,7 @@ def gemm_interval(a, b, bias, act: int, out_type: str, segs: int, device=None):
 # ------------------------------------------------------------------------------------------------ MLP head
 def mlp_head(X, coefs, intercepts, device=None):
     """The MLP head at device precision with interval propagation: X f32 -> bf16 (misc.cu convert_rows_vec_kernel),
-    weights bf16 (api.cu ie_mlp_load_layer), f32 accumulate + bias, relu, bf16 hidden store (gemm.cu pack_bf16x2), the
+    weights bf16 (api_mlp.cu ie_mlp_load_layer), f32 accumulate + bias, relu, bf16 hidden store (gemm.cu pack_bf16x2), the
     last layer sigmoid_acc on f32.  A hidden value whose interval straddles a bf16 rounding boundary may be either
     neighbour on the device; that uncertainty is carried into the next layer.
     Returns (p, lo, hi) float64 torch tensors [n, n_labels]: the device's probabilities must lie in [lo, hi]."""
@@ -603,7 +603,7 @@ def gemm_exact(a, b, bias, act: int, out_type: str, segs: int, gates=rounded_gat
 
 
 def mlp_head_exact(X, coefs, intercepts, gates=rounded_gates, device=None):
-    """The MLP head as ie_mlp_predict_proba (api.cu) computes it, bit for bit: X f32 -> bf16, weights f32 -> bf16,
+    """The MLP head as ie_mlp_predict_proba (api_mlp.cu) computes it, bit for bit: X f32 -> bf16, weights f32 -> bf16,
     each hidden layer relu(acc + bias) stored as bf16, the last layer sigmoid_acc of the f32 acc + bias.
     coefs [fan_in, fan_out] (sklearn layout), intercepts [fan_out].  Returns float64 [n, n_labels] (f32 values)."""
     x = _t(np.asarray(X, dtype=np.float32), device)

@@ -1,5 +1,5 @@
 """GPU tests of the similar-issue index where its fused top-k can go wrong (csrc/knn.cu, the ie_knn_* half of
-csrc/api.cu, code_intelligence_b200/knn.py): exact-arithmetic tie storms checked bit for bit, worst-case arrival orders,
+csrc/api_knn.cu, code_intelligence_b200/knn.py): exact-arithmetic tie storms checked bit for bit, worst-case arrival orders,
 permutation and power-of-two scale invariance, the norm range, the degraded regime, multi-pass searches, the largest
 merge, and lifecycle / stream / thread use of a handle.
 
